@@ -14,17 +14,29 @@
 //       expand    : 1/8 B mask + 2 B x density in, 2 B out
 // `values` is written into a caller buffer of capacity rows * cols; nnz stays on the device.
 //
-// Work decomposition (2-byte dtypes, cols % 8 == 0): unit = 8 elements = one 16-byte access and one mask byte; tile = 256 threads x
-// BM_U units, thread t owns units t + 256 u (coalesced), scan order = unit order.  The kept elements of a tile are staged in shared
-// memory so that the compact side is moved coalesced.
-#include <cstdlib>
+// Work decomposition (2-byte dtypes, cols % 8 == 0): unit = 8 elements = one 16-byte access and one mask byte; tile = 128 threads x 8
+// units, scan order = unit order.  The kept elements of a tile are staged in shared memory so that the compact side is moved coalesced.
+//
+// Why the kernels are shaped as they are:
+//   * One tile per CTA, its ticket taken when the CTA starts, so processing order is ticket order.  A CTA that claims a ticket ahead of
+//     its work (a persistent CTA that prefetches its next tile) publishes that tile's count late, and every successor waits for it.
+//   * The whole CTA looks back, politely: each predecessor's descriptor is read once per round, and a round is repeated after a
+//     nanosleep only while a descriptor that is actually needed is unpublished.  Threads that spin on their descriptors saturate the
+//     L2 and stretch the very round trip the prefix frontier advances by.
+//   * Compression publishes its tile's count as soon as it is known and collects its prefix only after the gather: by then the
+//     predecessors have mostly published, so the wait overlaps the tile's own work instead of preceding it.
+//   * A tile lives through mostly serial latencies (ticket, bulk load, barriers, descriptor read, write-out), so what counts is how
+//     many tiles an SM keeps in flight.  A scatter from a register-resident tile needs fewer instructions than the gather in shared
+//     memory, but 72 registers per thread instead of 32 (sm_90a) and so fewer CTAs per SM; measured on the B200 it was slower.
 
 #include "engine.h"
 
 namespace ctb {
 
-constexpr int BM_U = 4;
-constexpr int BM_TILE = 256 * BM_U;   // units per tile (8192 elements, 16 KB of bf16)
+constexpr int BM_THREADS = 128;                    // threads per CTA
+constexpr int BM_WARPS = BM_THREADS / 32;
+constexpr int BM_UPT = 8;                          // units per thread
+constexpr int BM_TILE = BM_UPT * BM_THREADS;       // units per tile (16 KB of bf16)
 
 constexpr unsigned long long DESC_A = 1ull << 62;   // value = this tile's count
 constexpr unsigned long long DESC_P = 2ull << 62;   // value = inclusive prefix up to and including this tile
@@ -39,238 +51,11 @@ __device__ __forceinline__ void st_desc(unsigned long long* p, unsigned long lon
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-__device__ __forceinline__ uint32_t nz_byte16(const uint4& v) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    uint32_t byte = 0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        byte |= ((w[j] & 0x7fffu) != 0u ? 1u : 0u) << (2 * j);            // -0.0 == 0
-        byte |= ((w[j] & 0x7fff0000u) != 0u ? 1u : 0u) << (2 * j + 1);
-    }
-    return byte;
-}
-
-// exclusive prefix of this tile = sum of the counts of tiles [0, tile); executed by warp 0.  `total` = this tile's count.
-__device__ __forceinline__ unsigned long long lookback(unsigned long long* desc, uint32_t tile, uint32_t total, int lane) {
-    if (lane == 0) st_desc(desc + tile, (tile == 0 ? DESC_P : DESC_A) | (unsigned long long)total);
-    unsigned long long excl = 0;
-    if (tile == 0) return 0;
-    int64_t look = (int64_t)tile - 1;          // lane l inspects tile look - l
-    while (true) {
-        const int64_t idx = look - lane;
-        unsigned long long d;
-        do {
-            d = (idx >= 0) ? ld_desc(desc + idx) : DESC_P;          // before the first tile: prefix 0
-        } while (__any_sync(0xffffffffu, (d >> 62) == 0));          // someone has not published yet: look again
-        const uint32_t has_p = __ballot_sync(0xffffffffu, (d >> 62) == 2);
-        // lanes up to (and including) the nearest tile that holds a prefix contribute
-        const int stop = has_p ? (__ffs(has_p) - 1) : 31;
-        unsigned long long part = (lane <= stop) ? (d & DESC_VAL) : 0ull;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        excl += part;
-        if (has_p) break;
-        look -= 32;
-    }
-    if (lane == 0) st_desc(desc + tile, DESC_P | (excl + total));
-    return excl;
-}
-
-// COMPRESS: src = dense [n_units x 16 B], dst = values (compact), bitmask written, row_offsets / nnz written
-// !COMPRESS: src = values (compact), bitmask read, dst = dense
-template <bool COMPRESS>
-__global__ void __launch_bounds__(256) bitmask_lookback_kernel(const void* __restrict__ src, uint8_t* __restrict__ bitmask, void* __restrict__ dst,
-                                                               int64_t* __restrict__ row_offsets, int64_t* __restrict__ nnz_out,
-                                                               unsigned long long* __restrict__ desc, uint32_t* __restrict__ ticket,
-                                                               uint32_t n_units, uint32_t n_tiles, FastDiv upr /* units per row */) {
-    __shared__ __align__(16) uint16_t stage[8 * BM_TILE];
-    __shared__ int warp_tot[BM_U][8];
-    __shared__ uint32_t tile_s;
-    __shared__ unsigned long long lb_sum[8];
-    __shared__ int lb_p[8];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) tile_s = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const uint32_t tile = tile_s;
-    if (tile >= n_tiles) return;
-    const uint32_t u0 = tile * BM_TILE;
-
-    uint4 v[BM_U];
-    uint32_t byte[BM_U];
-    int cnt[BM_U], incl[BM_U], off[BM_U];
-#pragma unroll
-    for (int u = 0; u < BM_U; ++u) {
-        const uint32_t i = u0 + u * 256 + threadIdx.x;
-        v[u] = make_uint4(0, 0, 0, 0);
-        byte[u] = 0;
-        if (i < n_units) {
-            if (COMPRESS) v[u] = ldg_stream16(reinterpret_cast<const uint4*>(src) + i);
-            else byte[u] = __ldg(bitmask + i);
-        }
-    }
-#pragma unroll
-    for (int u = 0; u < BM_U; ++u) {
-        if (COMPRESS) byte[u] = nz_byte16(v[u]);
-        cnt[u] = __popc(byte[u]);
-        incl[u] = cnt[u];
-    }
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-#pragma unroll
-        for (int u = 0; u < BM_U; ++u) {
-            const int n = __shfl_up_sync(0xffffffffu, incl[u], o);
-            if (lane >= o) incl[u] += n;
-        }
-    }
-    if (lane == 31) {
-#pragma unroll
-        for (int u = 0; u < BM_U; ++u) warp_tot[u][warp] = incl[u];
-    }
-    if (COMPRESS) {
-        // mask bytes: four neighbouring lanes combine theirs into one aligned 32-bit store (n_units % 4 == 0)
-#pragma unroll
-        for (int u = 0; u < BM_U; ++u) {
-            const uint32_t i = u0 + u * 256 + threadIdx.x;
-            uint32_t w = byte[u];
-            w |= __shfl_down_sync(0xffffffffu, w, 1) << 8;
-            w |= __shfl_down_sync(0xffffffffu, w, 2) << 16;
-            if ((threadIdx.x & 3) == 0 && i < n_units) reinterpret_cast<uint32_t*>(bitmask)[i >> 2] = w;
-        }
-    }
-    __syncthreads();
-    int total = 0;
-#pragma unroll
-    for (int u = 0; u < BM_U; ++u) {
-        int before = 0, seg = 0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) {
-            const int t = warp_tot[u][w];
-            if (w < warp) before += t;
-            seg += t;
-        }
-        off[u] = total + before + incl[u] - cnt[u];      // this unit's first slot in the tile's compact run
-        total += seg;
-    }
-    // stage first (tile-local offsets only), then the whole CTA looks back: 256 descriptors per step
-    if (COMPRESS) {
-#pragma unroll
-        for (int u = 0; u < BM_U; ++u) {
-            const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-            int o = off[u];
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-                if ((byte[u] >> k) & 1u) stage[o++] = (uint16_t)(w[k >> 1] >> (16 * (k & 1)));
-        }
-    }
-    if (threadIdx.x == 0) st_desc(desc + tile, (tile == 0 ? DESC_P : DESC_A) | (unsigned long long)total);
-    unsigned long long excl = 0;
-    if (tile > 0) {
-        int64_t base = (int64_t)tile - 1;
-        while (true) {
-            const int64_t idx = base - threadIdx.x;
-            unsigned long long d = DESC_P;                 // before the first tile: prefix 0
-            if (idx >= 0) {
-                do { d = ld_desc(desc + idx); } while ((d >> 62) == 0);
-            }
-            const uint32_t has_p = __ballot_sync(0xffffffffu, (d >> 62) == 2);
-            const int stop = has_p ? (__ffs(has_p) - 1) : 31;
-            unsigned long long part = (lane <= stop) ? (d & DESC_VAL) : 0ull;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-            if (lane == 0) { lb_sum[warp] = part; lb_p[warp] = has_p != 0; }
-            __syncthreads();
-            bool found = false;
-#pragma unroll
-            for (int w = 0; w < 8; ++w) {
-                if (!found) { excl += lb_sum[w]; found = lb_p[w] != 0; }
-            }
-            __syncthreads();
-            if (found) break;
-            base -= 256;
-        }
-    }
-    if (threadIdx.x == 0) {
-        st_desc(desc + tile, DESC_P | (excl + (unsigned long long)total));
-        if (COMPRESS && tile == n_tiles - 1) *nnz_out = (int64_t)(excl + (unsigned long long)total);
-    }
-    __syncthreads();
-    const unsigned long long pos = excl;
-    uint16_t* cout = reinterpret_cast<uint16_t*>(dst);
-    const uint16_t* cin = reinterpret_cast<const uint16_t*>(src);
-    // compact run [pos, pos + total): one 2-byte element to reach 4-byte alignment, then pairs, then a possible last element
-    const int head = (int)(pos & 1ull) & (total > 0 ? 1 : 0);     // values is at least 4-byte aligned: parity of the element index
-    const int pairs = (total - head) >> 1;
-    const int tail = total - head - 2 * pairs;
-    if (COMPRESS) {
-        if (row_offsets) {
-#pragma unroll
-            for (int u = 0; u < BM_U; ++u) {
-                const uint32_t i = u0 + u * 256 + threadIdx.x;
-                if (i < n_units) {
-                    const uint32_t r = fd_div(i, upr);
-                    if (r * upr.d == i) row_offsets[r] = (int64_t)(pos + (unsigned long long)off[u]);
-                }
-            }
-        }
-        if (threadIdx.x == 0 && head) cout[pos] = stage[0];
-        uint32_t* c32 = reinterpret_cast<uint32_t*>(cout + pos + head);
-        for (int j = threadIdx.x; j < pairs; j += 256) c32[j] = (uint32_t)stage[head + 2 * j] | ((uint32_t)stage[head + 2 * j + 1] << 16);
-        if (threadIdx.x == 32 && tail) cout[pos + total - 1] = stage[total - 1];
-    } else {
-        if (threadIdx.x == 0 && head) stage[0] = cin[pos];
-        const uint32_t* c32 = reinterpret_cast<const uint32_t*>(cin + pos + head);
-        for (int j = threadIdx.x; j < pairs; j += 256) {
-            const uint32_t two = ldg_stream4(c32 + j);
-            stage[head + 2 * j] = (uint16_t)two;
-            stage[head + 2 * j + 1] = (uint16_t)(two >> 16);
-        }
-        if (threadIdx.x == 32 && tail) stage[total - 1] = cin[pos + total - 1];
-        __syncthreads();
-#pragma unroll
-        for (int u = 0; u < BM_U; ++u) {
-            const uint32_t i = u0 + u * 256 + threadIdx.x;
-            if (i < n_units) {
-                uint32_t e[8];
-                int o = off[u];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) e[k] = ((byte[u] >> k) & 1u) ? (uint32_t)stage[o++] : 0u;
-                stg_stream16(reinterpret_cast<uint4*>(dst) + i, make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16)));
-            }
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------------------
-// The shipped kernels.  What the first versions taught:
-//   * v1 above (tile in registers, 64 registers -> 4 CTAs / SM, one warp looks back 32 descriptors per step): the prefix
-//     "frontier" advances one look-back window per L2 round trip.  The window, not the memory system, sets the speed.
-//   * widening the window to every thread of the CTA with a plain spin makes it worse: all threads re-reading
-//     their descriptor as fast as they can saturate the L2 and stretch the very round trip the frontier depends on.
-//   * a persistent CTA whose producer claims tickets AHEAD of the consumers (TMA ring) is wrong for a chained scan: a claimed tile
-//     that waits in the ring publishes nothing, and every successor in ticket order waits for it.
-// Hence: one tile per CTA, claimed when the CTA starts (processing order = ticket order); the tile lives in SHARED memory (one bulk
-// copy), so the kernel needs 40 registers and 6 CTAs / SM are resident; all 128 threads look back, but POLITELY -- one read per
-// descriptor per round, a round is repeated (after a nanosleep) only while a descriptor that is actually needed is unpublished.
-// ------------------------------------------------------------------------------------------------------------------------------
-#ifndef CT_BITMASK_THREADS
-#define CT_BITMASK_THREADS 128
-#endif
-// 128 threads x 8 units = 1024 units = 16 KB of input per tile.  With v5's LATE look-back a tile lives through mostly serial latencies
-// (ticket, bulk load, barriers, descriptor read, write-out), so what counts is how many tiles an SM has in flight: smaller tiles keep
-// more of them resident (CT_BITMASK_THREADS is the build-time knob)
-constexpr int B3_T = CT_BITMASK_THREADS;       // threads
-constexpr int B3_W = B3_T / 32;                // warps
-constexpr int B3_TILE = 8 * B3_T;              // units per tile
-constexpr int B3_UPT = B3_TILE / B3_T;         // units per thread (8)
-constexpr uint32_t B3_STAGE_BYTES = 8 * B3_TILE * 2 + 32;   // compact elements of a tile + one vector of slack for the funnel
-constexpr uint32_t B3_SMEM = 16 + B3_TILE * 16 + B3_STAGE_BYTES;
-
 __device__ __forceinline__ uint4 lds128(uint32_t saddr) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr));
     return v;
 }
-__device__ __forceinline__ void sts16(uint32_t saddr, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(saddr), "h"((unsigned short)v) : "memory"); }
 
 // exclusive prefix of `tile` (sum of the counts of all tiles before it); every thread of the CTA takes part and returns it.
 // Thread t inspects tile base - t; warp w therefore covers distances 32 w .. 32 w + 31, nearest first.
@@ -307,12 +92,12 @@ __device__ __forceinline__ unsigned long long lookback_cta(unsigned long long* d
         __syncthreads();
         bool found = false;
 #pragma unroll
-        for (int w = 0; w < B3_W; ++w) {
+        for (int w = 0; w < BM_WARPS; ++w) {
             if (!found) { excl += lb_sum[w]; found = lb_p[w] != 0; }
         }
         __syncthreads();
         if (found) break;
-        base -= B3_T;
+        base -= BM_THREADS;
     }
     if (threadIdx.x == 0) st_desc(desc + tile, DESC_P | (excl + (unsigned long long)total));
     return excl;
@@ -320,30 +105,30 @@ __device__ __forceinline__ unsigned long long lookback_cta(unsigned long long* d
 
 // per-thread scan bookkeeping shared by both directions: counts of the thread's 8 units (unit k * 128 + t, scan order = unit order)
 // -> off[k] = first slot of unit k in the tile's compact run; returns the tile's total
-__device__ __forceinline__ int tile_scan(const int (&cnt)[B3_UPT], int (&off)[B3_UPT], int (*warp_tot)[B3_W]) {
+__device__ __forceinline__ int tile_scan(const int (&cnt)[BM_UPT], int (&off)[BM_UPT], int (*warp_tot)[BM_WARPS]) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int incl[B3_UPT];
+    int incl[BM_UPT];
 #pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) incl[k] = cnt[k];
+    for (int k = 0; k < BM_UPT; ++k) incl[k] = cnt[k];
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
 #pragma unroll
-        for (int k = 0; k < B3_UPT; ++k) {
+        for (int k = 0; k < BM_UPT; ++k) {
             const int n = __shfl_up_sync(0xffffffffu, incl[k], o);
             if (lane >= o) incl[k] += n;
         }
     }
     if (lane == 31) {
 #pragma unroll
-        for (int k = 0; k < B3_UPT; ++k) warp_tot[k][warp] = incl[k];
+        for (int k = 0; k < BM_UPT; ++k) warp_tot[k][warp] = incl[k];
     }
     __syncthreads();
     int total = 0;
 #pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) {
+    for (int k = 0; k < BM_UPT; ++k) {
         int before = 0, seg = 0;
 #pragma unroll
-        for (int w = 0; w < B3_W; ++w) {
+        for (int w = 0; w < BM_WARPS; ++w) {
             const int t = warp_tot[k][w];
             if (w < warp) before += t;
             seg += t;
@@ -354,59 +139,13 @@ __device__ __forceinline__ int tile_scan(const int (&cnt)[B3_UPT], int (&off)[B3
     return total;
 }
 
-// the compact run [excl, excl + total) <-> the staging buffer, as 16-byte vectors aligned to GLOBAL 16-byte boundaries.  The run starts at
-// an arbitrary element, so global vector c corresponds to stage elements [8c - shift, 8c - shift + 8): cut out of the aligned shared
-// vectors c - 1 and c with a funnel shift (shift is tile-uniform).  TO_GLOBAL: stage -> values; else values -> stage (shifted copy:
-// global vector c lands at stage vector c, i.e. run element j at stage element j + shift).
-__device__ __forceinline__ void run_to_global(uint16_t* values, unsigned long long excl, int total, uint32_t stage0) {
-    const uint32_t shift = (uint32_t)(excl & 7ull);               // elements of the first global vector that belong to earlier tiles
-    const unsigned long long g0 = excl - shift;
-    const uint32_t span = shift + (uint32_t)total;
-    const uint32_t nvec = (span + 7) >> 3;
-    uint4* gv = reinterpret_cast<uint4*>(values + g0);
-    const uint32_t h0 = 8u - shift;                                // first half of the (vector c - 1, vector c) pair: 1 .. 8
-    const uint32_t wo = h0 >> 1, odd = h0 & 1u;
-    for (uint32_t c = threadIdx.x; c < nvec; c += B3_T) {
-        const bool first = (c == 0), last = (8 * c + 8 > span);
-        uint32_t o[4];
-        if (shift == 0) {
-            const uint4 A = lds128(stage0 + 16u * c);
-            o[0] = A.x; o[1] = A.y; o[2] = A.z; o[3] = A.w;
-        } else {
-            uint4 A = make_uint4(0, 0, 0, 0);
-            if (c > 0) A = lds128(stage0 + 16u * (c - 1));
-            const uint4 B = lds128(stage0 + 16u * c);
-            const uint32_t W[8] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                uint32_t lo, hi;
-                switch (wo) {                                       // tile-uniform; h0 in 1 .. 7 here, so wo in 0 .. 3
-                case 0: lo = W[i]; hi = W[i + 1]; break;
-                case 1: lo = W[i + 1]; hi = W[i + 2]; break;
-                case 2: lo = W[i + 2]; hi = W[i + 3]; break;
-                default: lo = W[i + 3]; hi = W[i + 4]; break;
-                }
-                o[i] = odd ? __funnelshift_r(lo, hi, 16) : lo;
-            }
-        }
-        if (!first && !last) stg_stream16(gv + c, make_uint4(o[0], o[1], o[2], o[3]));
-        else {
-            // partial vector: the elements before the run belong to the previous tile, those after it to the next one
-            uint16_t* ge = values + g0 + 8ull * c;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const uint32_t pos = 8 * c + e;
-                if (pos >= shift && pos < span) ge[e] = (uint16_t)(o[e >> 1] >> (16 * (e & 1)));
-            }
-        }
-    }
-}
-
-// The same write-out with the window of a global vector fetched as five 4-byte words from the 4-byte boundary at or below its first
-// element (one funnel shift by 16 when the run position is odd) instead of two 16-byte vectors and a tile-uniform `switch` over the
-// word offset, which the compiler turns into a select tree (8 % of v5's instructions).  May read up to 16 bytes BELOW stage0 (vector 0
-// of a run that does not start on a 16-byte boundary; those halves are never stored): the caller's buffer is preceded by >= 16 bytes
-// of its own shared memory.
+// the compact run [excl, excl + total) from the staging buffer (run element j at stage element j) to `values`, as 16-byte vectors aligned
+// to GLOBAL 16-byte boundaries.  The run starts at an arbitrary element, so global vector c holds stage elements [8c - shift, 8c - shift + 8)
+// (shift = excl mod 8, tile-uniform); its first and last vector are stored element by element, because their other elements belong to
+// the neighbouring tiles.  A vector's window is fetched as five 4-byte words from the 4-byte boundary at or below its first element (one
+// funnel shift by 16 when the run position is odd); two 16-byte loads and a switch over the word offset compile to a select tree.  May
+// read up to 16 bytes BELOW stage0 (vector 0 of a run that does not start on a 16-byte boundary; those halves are never stored): the
+// caller's buffer is preceded by >= 16 bytes of its own shared memory.
 __device__ __forceinline__ void run_to_global_words(uint16_t* values, unsigned long long excl, int total, uint32_t stage0) {
     const uint32_t shift = (uint32_t)(excl & 7ull);
     const unsigned long long g0 = excl - shift;
@@ -415,7 +154,7 @@ __device__ __forceinline__ void run_to_global_words(uint16_t* values, unsigned l
     uint4* gv = reinterpret_cast<uint4*>(values + g0);
     const uint32_t sh = (shift & 1u) << 4;
     const uint32_t base = stage0 - 2u * shift - 2u * (shift & 1u);        // word that holds stage element -shift (4-byte aligned)
-    for (uint32_t c = threadIdx.x; c < nvec; c += B3_T) {
+    for (uint32_t c = threadIdx.x; c < nvec; c += BM_THREADS) {
         const bool first = (c == 0), last = (8 * c + 8 > span);
         const uint32_t a = base + 16u * c;
         uint32_t w[5], o[4];
@@ -435,99 +174,6 @@ __device__ __forceinline__ void run_to_global_words(uint16_t* values, unsigned l
     }
 }
 
-__global__ void __launch_bounds__(B3_T) bitmask_compress_tile_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ bitmask,
-                                                                     uint16_t* __restrict__ values, int64_t* __restrict__ row_offsets,
-                                                                     int64_t* __restrict__ nnz_out, unsigned long long* __restrict__ desc,
-                                                                     uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles, FastDiv upr) {
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    __shared__ int warp_tot[B3_UPT][B3_W];
-    __shared__ unsigned long long lb_sum[B3_W];
-    __shared__ int lb_p[B3_W];
-    __shared__ uint32_t tile_s;
-    const uint32_t sbase = smem_u32(smem_raw);
-    const uint32_t bar = sbase, data = sbase + 16, stage0 = data + B3_TILE * 16;
-    const int tid = threadIdx.x;
-    if (tid == 0) {
-        // the ticket is taken when the CTA starts running: processing order = ticket order, every predecessor is resident or done
-        const uint32_t tile = atomicAdd(ticket, 1u);
-        tile_s = tile;
-        mbar_init_a(bar, 1);
-        mbar_fence_init();
-        const uint32_t nu = min((uint32_t)B3_TILE, n_units - tile * B3_TILE);
-        mbar_expect_tx_a(bar, nu * 16);
-        bulk_g2s_a(data, src + (size_t)tile * (B3_TILE * 16), nu * 16, bar, l2_evict_first_policy());
-    }
-    __syncthreads();
-    const uint32_t tile = tile_s;
-    const uint32_t u0 = tile * B3_TILE;
-    const uint32_t nu = min((uint32_t)B3_TILE, n_units - u0);
-    mbar_wait_a(bar, 0);
-
-    // ---- mask bytes, counts, scan ----
-    uint32_t bytes_lo = 0, bytes_hi = 0;      // mask bytes of units k = 0..3 / 4..7
-    int cnt[B3_UPT], off[B3_UPT];
-#pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) {
-        const uint32_t i = k * B3_T + tid;
-        uint32_t b = 0;
-        if (i < nu) b = nz_byte16(lds128(data + i * 16));
-        if (k < 4) bytes_lo |= b << (8 * k);
-        else bytes_hi |= b << (8 * (k - 4));
-        cnt[k] = __popc(b);
-        // four neighbouring lanes combine their bytes into one aligned 32-bit store (n_units % 4 == 0)
-        uint32_t w = b;
-        w |= __shfl_down_sync(0xffffffffu, w, 1) << 8;
-        w |= __shfl_down_sync(0xffffffffu, w, 2) << 16;
-        if ((tid & 3) == 0 && i < nu) reinterpret_cast<uint32_t*>(bitmask)[(u0 + i) >> 2] = w;
-    }
-    const int total = tile_scan(cnt, off, warp_tot);
-
-    // ---- compaction into the staging buffer (element j of the tile's run at stage[j]) ----
-#pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) {
-        const uint32_t i = k * B3_T + tid;
-        const uint32_t b = (k < 4 ? bytes_lo >> (8 * k) : bytes_hi >> (8 * (k - 4))) & 0xffu;
-        if (b) {
-            const uint4 v = lds128(data + i * 16);
-            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-            uint32_t o = stage0 + 2u * (uint32_t)off[k];
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if ((b >> e) & 1u) { sts16(o, w[e >> 1] >> (16 * (e & 1))); o += 2; }
-        }
-    }
-    // (the look-back's barriers also order the staging writes before the write-out)
-    const unsigned long long excl = lookback_cta(desc, tile, (uint32_t)total, lb_sum, lb_p);
-    if (tid == 0 && tile == n_tiles - 1) *nnz_out = (int64_t)(excl + (unsigned long long)total);
-    if (tile == 0) __syncthreads();            // tile 0 skips the look-back's barriers
-
-    if (row_offsets) {
-#pragma unroll
-        for (int k = 0; k < B3_UPT; ++k) {
-            const uint32_t i = k * B3_T + tid;
-            if (i < nu) {
-                const uint32_t gu = u0 + i, r = fd_div(gu, upr);
-                if (r * upr.d == gu) row_offsets[r] = (int64_t)(excl + (unsigned long long)off[k]);
-            }
-        }
-    }
-    run_to_global(values, excl, total, stage0);
-}
-
-// ------------------------------------------------------------------------------------------------------------------------------
-// v4 of the compressing direction: the same tile / ticket / look-back structure, but the compaction is a GATHER.
-// v3 (bitmask_compress_tile_kernel above) spends 25 instructions per input element and is bound by instruction issue: 8 units per thread in STRIDED order cost 40 scan shuffles and
-// 8 offset computations per thread, the non-zero byte 3 instructions per element, and every kept element is extracted, stored to a
-// staging buffer with a predicated 16-bit store, and read again for the write-out.
-//   * a thread owns 8 CONSECUTIVE units (64 elements): one count per thread -> 5 scan shuffles; its 8 mask bytes are one 8-byte store
-//   * non-zero byte of a unit: |x| != 0 per half with the packed 16-bit integer min (VIMNMX.U16x2 against 0x00010001): 13 instructions
-//   * no staging buffer: after the look-back every thread knows where the tile's run starts in `values`; OUTPUT vector v (8 kept
-//     elements, 16 bytes, aligned in global memory) is produced by one thread that walks the tile's bit mask from the position of the
-//     vector's first element (a 2 KB table filled by the threads that own those positions) and fetches the kept halves straight from
-//     the tile in shared memory
-// ------------------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t B4_SMEM = 16 + B3_TILE * 16;
-
 // non-zero byte of 8 halves: per word  min(|x| per half, 1)  ->  bit 0 / bit 16; folded into 8 bits
 __device__ __forceinline__ uint32_t nz_byte16_fast(const uint4& v) {
     const uint32_t r0 = __vminu2(v.x & 0x7fff7fffu, 0x00010001u), r1 = __vminu2(v.y & 0x7fff7fffu, 0x00010001u);
@@ -541,27 +187,27 @@ __device__ __forceinline__ uint32_t byte_popc4(uint32_t x) {
     x = (x & 0x33333333u) + ((x >> 2) & 0x33333333u);
     return (x + (x >> 4)) & 0x0f0f0f0fu;
 }
-// position of the n-th (0-based) set bit of x; x has more than n set bits
-__device__ __forceinline__ uint32_t select32(uint32_t x, uint32_t n) {
-    uint32_t pos = 0;
-#pragma unroll
-    for (int w = 16; w >= 1; w >>= 1) {
-        const uint32_t c = __popc(x & ((1u << w) - 1u));
-        if (n >= c) { n -= c; x >>= w; pos += w; }
-    }
-    return pos;
-}
 
-__global__ void __launch_bounds__(B3_T) bitmask_compress_gather_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ bitmask,
-                                                                       uint16_t* __restrict__ values, int64_t* __restrict__ row_offsets,
-                                                                       int64_t* __restrict__ nnz_out, unsigned long long* __restrict__ desc,
-                                                                       uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles, FastDiv upr) {
+// ------------------------------------------------------------------------------------------------------------------------------
+// Compression.  The tile arrives in shared memory with one bulk copy; thread t owns its 8 consecutive units 8 t .. 8 t + 7.
+//   A: mask bytes, the thread's count, the CTA scan; the tile's count is published at once.
+//   B: the tile's run is cut into vectors of 8 kept elements, aligned to the start of the RUN (not to global 16-byte boundaries, which
+//      would need the prefix); the thread that owns a vector's first element records where that element sits in the tile.
+//   C: one thread per vector walks the mask from there and gathers its 8 kept elements, compacting the tile in place.
+//   D: the prefix (published by now), row offsets, and the write-out of the run to globally aligned vectors (run_to_global_words).
+// ------------------------------------------------------------------------------------------------------------------------------
+constexpr uint32_t BM_SMEM = 16 + BM_TILE * 16 + 32;    // + two vectors of slack: the write-out reads up to one vector past the run
+
+__global__ void __launch_bounds__(BM_THREADS) bitmask_compress_late_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ bitmask,
+                                                                           uint16_t* __restrict__ values, int64_t* __restrict__ row_offsets,
+                                                                           int64_t* __restrict__ nnz_out, unsigned long long* __restrict__ desc,
+                                                                           uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles, FastDiv upr) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
-    __shared__ __align__(16) uint32_t mask_w[B3_TILE / 4 + 4];   // the tile's mask bytes (+ zero padding for the walkers' look-ahead)
-    __shared__ uint16_t start_s[B3_TILE + 8];                     // element index (within the tile) of the first element of output vector v
-    __shared__ int warp_tot[B3_W];
-    __shared__ unsigned long long lb_sum[B3_W];
-    __shared__ int lb_p[B3_W];
+    __shared__ __align__(16) uint32_t mask_w[BM_TILE / 4 + 4];   // the tile's mask bytes (+ zero padding for the walkers' look-ahead)
+    __shared__ uint16_t start_s[BM_TILE + 8];                     // element index (within the tile) of the first element of run vector v
+    __shared__ int warp_tot[BM_WARPS];
+    __shared__ unsigned long long lb_sum[BM_WARPS];
+    __shared__ int lb_p[BM_WARPS];
     __shared__ uint32_t tile_s;
     const uint32_t sbase = smem_u32(smem_raw);
     const uint32_t bar = sbase, data = sbase + 16;
@@ -571,194 +217,25 @@ __global__ void __launch_bounds__(B3_T) bitmask_compress_gather_kernel(const uin
         tile_s = tile;
         mbar_init_a(bar, 1);
         mbar_fence_init();
-        const uint32_t nu = min((uint32_t)B3_TILE, n_units - tile * B3_TILE);
+        const uint32_t nu = min((uint32_t)BM_TILE, n_units - tile * BM_TILE);
         mbar_expect_tx_a(bar, nu * 16);
-        bulk_g2s_a(data, src + (size_t)tile * (B3_TILE * 16), nu * 16, bar, l2_evict_first_policy());
+        bulk_g2s_a(data, src + (size_t)tile * (BM_TILE * 16), nu * 16, bar, l2_evict_first_policy());
     }
-    if (tid < 4) mask_w[B3_TILE / 4 + tid] = 0u;
+    if (tid < 4) mask_w[BM_TILE / 4 + tid] = 0u;
     __syncthreads();
     const uint32_t tile = tile_s;
-    const uint32_t u0 = tile * B3_TILE;
-    const uint32_t nu = min((uint32_t)B3_TILE, n_units - u0);
+    const uint32_t u0 = tile * BM_TILE;
+    const uint32_t nu = min((uint32_t)BM_TILE, n_units - u0);
     mbar_wait_a(bar, 0);
 
-    // ---- A: mask bytes of the thread's 8 consecutive units (read in a lane-dependent order: bank-conflict free), counts, scan ----
+    // ---- A: mask bytes of the thread's 8 consecutive units, counts, scan ----
     const uint32_t uf = 8u * (uint32_t)tid;
     uint8_t* mask_b = reinterpret_cast<uint8_t*>(mask_w);
     {
         const uint32_t sw = (uint32_t)(tid & 7);
         const uint32_t tdata = data + uf * 16;
         uint8_t* tmask = mask_b + uf;
-        if (nu == (uint32_t)B3_TILE) {                 // a full tile (all but the last one): no bounds checks
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const uint32_t p = (uint32_t)k ^ sw;
-                tmask[p] = (uint8_t)nz_byte16_fast(lds128(tdata + p * 16));
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const uint32_t p = (uint32_t)k ^ sw;
-                uint32_t b = 0;
-                if (uf + p < nu) b = nz_byte16_fast(lds128(tdata + p * 16));
-                tmask[p] = (uint8_t)b;
-            }
-        }
-    }
-    const uint32_t lo = mask_w[2 * tid], hi = mask_w[2 * tid + 1];       // written by this thread: no barrier needed
-    if (uf + 4 <= nu) reinterpret_cast<uint32_t*>(bitmask + u0 + uf)[0] = lo;        // n_units % 4 == 0; the mask is 4-byte aligned
-    if (uf + 8 <= nu) reinterpret_cast<uint32_t*>(bitmask + u0 + uf)[1] = hi;
-    const int clo = __popc(lo), cnt = clo + __popc(hi);
-    int incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int n = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += n;
-    }
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();                                                       // also publishes every thread's mask bytes
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < B3_W; ++w) {
-        const int t = warp_tot[w];
-        if (w < warp) before += t;
-        total += t;
-    }
-    const int toff = before + incl - cnt;          // first slot of this thread's elements in the tile's run
-
-    const unsigned long long excl = lookback_cta(desc, tile, (uint32_t)total, lb_sum, lb_p);
-    if (tid == 0 && tile == n_tiles - 1) *nnz_out = (int64_t)(excl + (unsigned long long)total);
-
-    // ---- row offsets: a row starts in this thread's units at most once when a row has >= 8 units ----
-    if (row_offsets && uf < nu) {
-        const uint32_t g = u0 + uf;
-        uint32_t r = fd_div(g, upr);
-        uint32_t k = (r * upr.d == g) ? 0u : (r + 1) * upr.d - g;          // units until the next row start
-        if (k != 0) ++r;
-        while (k < 8 && uf + k < nu) {
-            const uint32_t below = (k < 4) ? __popc(lo & ((1u << (8 * k)) - 1u)) : (uint32_t)clo + __popc(hi & ((1u << (8 * (k - 4))) - 1u));
-            row_offsets[r] = (int64_t)(excl + (unsigned long long)toff + below);
-            k += upr.d;
-            ++r;
-        }
-    }
-
-    // ---- B: where does output vector v start?  run element j0(v) = max(8 v - shift, 0); the thread that owns it records its position ----
-    const uint32_t shift = (uint32_t)(excl & 7ull);
-    const uint32_t span = shift + (uint32_t)total;
-    const uint32_t nvec = (span + 7) >> 3;
-    if (cnt > 0) {
-        uint32_t v = ((uint32_t)toff + shift + 7) >> 3;                     // first vector whose first element is at or after toff
-        if (toff == 0) v = 0;
-        while (true) {
-            const uint32_t j0 = (v == 0) ? 0u : 8 * v - shift;
-            if (j0 >= (uint32_t)(toff + cnt)) break;
-            const uint32_t n = j0 - (uint32_t)toff;
-            const uint32_t bit = (n < (uint32_t)clo) ? select32(lo, n) : 32u + select32(hi, n - (uint32_t)clo);
-            start_s[v] = (uint16_t)(uf * 8 + bit);
-            ++v;
-        }
-    }
-    __syncthreads();
-
-    // ---- C: one thread per output vector walks the mask from the vector's first element and gathers 8 kept halves from the tile ----
-    const unsigned long long g0 = excl - shift;
-    for (uint32_t v = tid; v < nvec; v += B3_T) {
-        const uint32_t p_lo = (v == 0) ? shift : 0u;                         // positions of this vector that belong to the run
-        const uint32_t p_hi = min(8u, span - 8 * v);
-        if (p_lo >= p_hi) continue;                                          // an empty tile's only vector: nothing of it belongs to this run
-        uint32_t bit = start_s[v];
-        uint32_t wi = bit >> 5;
-        const uint32_t s = bit & 31u;
-        uint32_t cur = __funnelshift_r(mask_w[wi], mask_w[wi + 1], s);      // kept-flags of elements bit .. bit + 31
-        uint32_t ebase = data + bit * 2;                                     // shared address of element `bit`
-        if (p_lo == 0 && p_hi == 8) {
-            // the common case: a whole vector.  Per element: isolate the lowest kept flag, its position, one 16-bit shared load
-            uint32_t h[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                while (cur == 0u) {                                          // the next kept element is further than 32 positions away
-                    ++wi;
-                    ebase += 64;
-                    cur = __funnelshift_r(mask_w[wi], mask_w[wi + 1], s);
-                }
-                const uint32_t pos = (uint32_t)__ffs(cur) - 1u;
-                cur &= cur - 1u;
-                unsigned short t;
-                asm volatile("ld.shared.u16 %0, [%1];" : "=h"(t) : "r"(ebase + 2 * pos));
-                h[e] = t;
-            }
-            stg_stream16(reinterpret_cast<uint4*>(values + g0) + v,
-                         make_uint4(h[0] | (h[1] << 16), h[2] | (h[3] << 16), h[4] | (h[5] << 16), h[6] | (h[7] << 16)));
-        } else {
-            // the run's first / last vector: only positions [p_lo, p_hi) are ours
-            uint16_t* ge = values + g0 + 8ull * v;
-            for (uint32_t e = p_lo; e < p_hi; ++e) {
-                while (cur == 0u) {
-                    ++wi;
-                    ebase += 64;
-                    cur = __funnelshift_r(mask_w[wi], mask_w[wi + 1], s);
-                }
-                const uint32_t pos = (uint32_t)__ffs(cur) - 1u;
-                cur &= cur - 1u;
-                unsigned short t;
-                asm volatile("ld.shared.u16 %0, [%1];" : "=h"(t) : "r"(ebase + 2 * pos));
-                ge[e] = t;
-            }
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------------------
-// v5 (shipped): v4 with the look-back moved BEHIND the gather.  In v4 a large share of the stalls sit
-// in lookback_cta -- a CTA finishes its counts and then waits until every predecessor of its window has finished ITS counts, i.e.
-// for the slowest of up to 256 bulk loads that were issued at about the same time; nothing of the tile's own work can proceed,
-// because v4 lays its output vectors on GLOBAL 16-byte boundaries and therefore needs (prefix mod 8) before it gathers.
-// Here the vectors are laid on the boundaries of the tile's OWN run: the aggregate is published as soon as it is known, the gather
-// compacts the tile in place in shared memory (vector v of the run over elements 8 v .. 8 v + 7 of the tile; sources are never below
-// their destination, one barrier per pass of one vector per thread separates a pass's reads from its writes), and only then the prefix is
-// collected -- by now it is there -- and the run leaves through the funnel-shifted, globally aligned write-out of v3.
-// ------------------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t B5_SMEM = 16 + B3_TILE * 16 + 32;    // + two vectors of slack: the write-out reads up to one vector past the run
-
-__global__ void __launch_bounds__(B3_T) bitmask_compress_late_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ bitmask,
-                                                                     uint16_t* __restrict__ values, int64_t* __restrict__ row_offsets,
-                                                                     int64_t* __restrict__ nnz_out, unsigned long long* __restrict__ desc,
-                                                                     uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles, FastDiv upr) {
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    __shared__ __align__(16) uint32_t mask_w[B3_TILE / 4 + 4];   // the tile's mask bytes (+ zero padding for the walkers' look-ahead)
-    __shared__ uint16_t start_s[B3_TILE + 8];                     // element index (within the tile) of the first element of run vector v
-    __shared__ int warp_tot[B3_W];
-    __shared__ unsigned long long lb_sum[B3_W];
-    __shared__ int lb_p[B3_W];
-    __shared__ uint32_t tile_s;
-    const uint32_t sbase = smem_u32(smem_raw);
-    const uint32_t bar = sbase, data = sbase + 16;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) {
-        const uint32_t tile = atomicAdd(ticket, 1u);
-        tile_s = tile;
-        mbar_init_a(bar, 1);
-        mbar_fence_init();
-        const uint32_t nu = min((uint32_t)B3_TILE, n_units - tile * B3_TILE);
-        mbar_expect_tx_a(bar, nu * 16);
-        bulk_g2s_a(data, src + (size_t)tile * (B3_TILE * 16), nu * 16, bar, l2_evict_first_policy());
-    }
-    if (tid < 4) mask_w[B3_TILE / 4 + tid] = 0u;
-    __syncthreads();
-    const uint32_t tile = tile_s;
-    const uint32_t u0 = tile * B3_TILE;
-    const uint32_t nu = min((uint32_t)B3_TILE, n_units - u0);
-    mbar_wait_a(bar, 0);
-
-    // ---- A: mask bytes of the thread's 8 consecutive units, counts, scan (as v4) ----
-    const uint32_t uf = 8u * (uint32_t)tid;
-    uint8_t* mask_b = reinterpret_cast<uint8_t*>(mask_w);
-    {
-        const uint32_t sw = (uint32_t)(tid & 7);
-        const uint32_t tdata = data + uf * 16;
-        uint8_t* tmask = mask_b + uf;
-        if (nu == (uint32_t)B3_TILE) {
+        if (nu == (uint32_t)BM_TILE) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
                 const uint32_t p = (uint32_t)k ^ sw;
@@ -788,7 +265,7 @@ __global__ void __launch_bounds__(B3_T) bitmask_compress_late_kernel(const uint8
     __syncthreads();
     int before = 0, total = 0;
 #pragma unroll
-    for (int w = 0; w < B3_W; ++w) {
+    for (int w = 0; w < BM_WARPS; ++w) {
         const int t = warp_tot[w];
         if (w < warp) before += t;
         total += t;
@@ -827,7 +304,7 @@ __global__ void __launch_bounds__(B3_T) bitmask_compress_late_kernel(const uint8
     // ---- C: gather, in place.  Pass k: vectors T k .. T k + T - 1 (T threads) are read into registers, barrier, written to elements 8 v .. 8 v + 7.
     // A source element is never below its destination, and the sources of LATER passes lie at or above the end of this pass's
     // destinations, so one barrier per pass is enough.
-    for (uint32_t vb = 0; vb < nvec; vb += B3_T) {
+    for (uint32_t vb = 0; vb < nvec; vb += BM_THREADS) {
         const uint32_t v = vb + (uint32_t)tid;
         uint32_t h[8];
 #pragma unroll
@@ -897,193 +374,35 @@ __global__ void __launch_bounds__(B3_T) bitmask_compress_late_kernel(const uint8
     run_to_global_words(values, excl, total, data);
 }
 
-// ------------------------------------------------------------------------------------------------------------------------------
-// v6 (NOT shipped; CT_B200_BITMASK_V6=1): what the expanding direction taught (csrc/sparse.cu, bitmask_expand_rows_kernel), applied here.  v5 is bound by
-// instruction issue, and 62 % of its instructions serve the GATHER formulation (a table of where every output vector starts, then a
-// walk over the bit mask per kept element: ~19 instructions per kept element).  A SCATTER needs ~3 per input element whatever the
-// density (extract the half, predicated 16-bit shared store, bump the offset) -- v3 did that and drowned in scan bookkeeping.  Here:
-//   * the tile never sits in shared memory: a thread loads its 8 units (i = u * 256 + tid: consecutive lanes own consecutive units, so
-//     their kept runs are ~2 words apart in the staging buffer and the 16-bit stores do not collide in the banks) with 8 independent
-//     16-byte loads and keeps them in registers (32 KB in flight per CTA, as the bulk copy had)
-//   * the eight per-slot warp scans run two 16-bit counters per register (20 shuffles instead of 40); the eight warp totals of every
-//     slot are scanned by lanes 0-7 with three shuffle rounds, not by 32 loads + selects in every thread
-//   * the aggregate is published as soon as it is known, the look-back runs BEHIND the compaction (v5), the run leaves through v3's
-//     funnel-shifted, globally aligned write-out
-//   * persistent CTAs: the next tile's ticket is taken and its loads are issued before the current tile's look-back and write-out
-// It is slower than v5 in both forms.  Fewer instructions (14 per element instead of 21) do not help: a tile lives through mostly serial
-// latencies (ticket, load, two barriers, descriptor read, write-out), 64-78 registers allow 3-4 CTAs / SM instead of 5, and the persistent form repeats v2's
-// lesson -- a ticket taken ahead of the work publishes its aggregate late and every successor in ticket order waits for it.
-// ------------------------------------------------------------------------------------------------------------------------------
-constexpr int B6_NP = B3_UPT / 2;
-constexpr uint32_t B6_SMEM = 8 * B3_TILE * 2 + 64;     // the compact run of a full tile + the vector the write-out may read past it
-static_assert(B3_W <= 8 && B3_UPT == 8, "the warp-total scan runs on lanes 0 .. 7");
-
-__global__ void __launch_bounds__(B3_T, 3) bitmask_compress_regs_kernel(const uint4* __restrict__ src, uint8_t* __restrict__ bitmask,
-                                                                        uint16_t* __restrict__ values, int64_t* __restrict__ row_offsets,
-                                                                        int64_t* __restrict__ nnz_out, unsigned long long* __restrict__ desc,
-                                                                        uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles, FastDiv upr) {
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    __shared__ __align__(16) uint32_t mask_w[B3_TILE / 4];
-    __shared__ uint32_t warp_tot[B6_NP][B3_W];
-    __shared__ unsigned long long lb_sum[B3_W];
-    __shared__ int lb_p[B3_W];
-    __shared__ uint32_t tile_s[2];
-    const uint32_t stage0 = smem_u32(smem_raw);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) tile_s[0] = atomicAdd(ticket, 1u);   // taken when the work on it starts: processing order = ticket order
-    __syncthreads();
-    uint32_t tile = tile_s[0];
-    if (tile >= n_tiles) return;
-    uint32_t u0 = tile * B3_TILE;
-    uint32_t nu = min((uint32_t)B3_TILE, n_units - u0);
-
-    // ---- the tile: 8 independent 16-byte loads per thread ----
-    uint4 v[B3_UPT];
-#pragma unroll
-    for (int u = 0; u < B3_UPT; ++u) {
-        const uint32_t i = (uint32_t)u * B3_T + (uint32_t)tid;
-        v[u] = (i < nu) ? ldg_stream16(src + u0 + i) : make_uint4(0, 0, 0, 0);
-    }
-    for (uint32_t it = 0;; ++it) {
-        // ---- mask bytes, counts (two per register), warp scans ----
-        uint32_t blo = 0, bhi = 0, pk[B6_NP];
-        uint8_t* mask_b = reinterpret_cast<uint8_t*>(mask_w);
-#pragma unroll
-        for (int i = 0; i < B6_NP; ++i) pk[i] = 0u;
-#pragma unroll
-        for (int u = 0; u < B3_UPT; ++u) {
-            const uint32_t b = nz_byte16_fast(v[u]);
-            mask_b[u * B3_T + tid] = (uint8_t)b;
-            if (u < 4) blo |= b << (8 * u);
-            else bhi |= b << (8 * (u - 4));
-            pk[u >> 1] |= (uint32_t)__popc(b) << (16 * (u & 1));
-        }
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-#pragma unroll
-            for (int i = 0; i < B6_NP; ++i) {
-                const uint32_t n = __shfl_up_sync(0xffffffffu, pk[i], o);
-                if (lane >= o) pk[i] += n;
-            }
-        }
-        if (lane == 31) {
-#pragma unroll
-            for (int i = 0; i < B6_NP; ++i) warp_tot[i][warp] = pk[i];
-        }
-        __syncthreads();                                   // warp totals and every thread's mask bytes
-        // the NEXT tile's ticket: its latency hides behind the compaction; every thread reads it after the barrier below
-        if (tid == 0) tile_s[(it + 1) & 1] = atomicAdd(ticket, 1u);
-        // the tile's mask bytes leave as two coalesced 4-byte words per thread (n_units % 4 == 0)
-        {
-            const uint32_t uf = 8u * (uint32_t)tid;
-            if (uf + 4 <= nu) reinterpret_cast<uint32_t*>(bitmask + u0 + uf)[0] = mask_w[2 * tid];
-            if (uf + 8 <= nu) reinterpret_cast<uint32_t*>(bitmask + u0 + uf)[1] = mask_w[2 * tid + 1];
-        }
-        int off[B3_UPT];
-        int total = 0;
-        {
-            uint32_t t[B6_NP], before[B6_NP], seg[B6_NP];
-#pragma unroll
-            for (int i = 0; i < B6_NP; ++i) t[i] = (lane < B3_W) ? warp_tot[i][lane] : 0u;
-#pragma unroll
-            for (int o = 1; o < 8; o <<= 1) {
-#pragma unroll
-                for (int i = 0; i < B6_NP; ++i) {
-                    const uint32_t n = __shfl_up_sync(0xffffffffu, t[i], o);
-                    if (lane >= o) t[i] += n;
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < B6_NP; ++i) {
-                before[i] = __shfl_sync(0xffffffffu, t[i], (warp + 31) & 31);
-                if (warp == 0) before[i] = 0u;
-                seg[i] = __shfl_sync(0xffffffffu, t[i], B3_W - 1);
-            }
-#pragma unroll
-            for (int u = 0; u < B3_UPT; ++u) {
-                const int sh = 16 * (u & 1);
-                const uint32_t b = (u < 4 ? blo >> (8 * u) : bhi >> (8 * (u - 4))) & 0xffu;
-                off[u] = total + (int)((before[u >> 1] >> sh) & 0xffffu) + (int)((pk[u >> 1] >> sh) & 0xffffu) - __popc(b);
-                total += (int)((seg[u >> 1] >> sh) & 0xffffu);
-            }
-        }
-        lookback_publish(desc, tile, (uint32_t)total);        // the successors' look-back can pass this tile from here on
-
-        // ---- compaction from the registers into the staging buffer (element j of the tile's run at stage[j]) ----
-#pragma unroll
-        for (int u = 0; u < B3_UPT; ++u) {
-            const uint32_t b = (u < 4 ? blo >> (8 * u) : bhi >> (8 * (u - 4))) & 0xffu;
-            const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-            uint32_t o = stage0 + 2u * (uint32_t)off[u];
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if ((b >> e) & 1u) { sts16(o, w[e >> 1] >> (16 * (e & 1))); o += 2; }
-        }
-        __syncthreads();
-
-        // ---- the registers are free: the next tile's loads fly while this tile's prefix is collected and its run written out ----
-        const uint32_t next = tile_s[(it + 1) & 1];
-        const uint32_t nu0 = u0, nun = nu;
-        const bool more = next < n_tiles;
-        if (more) {
-            u0 = next * B3_TILE;
-            nu = min((uint32_t)B3_TILE, n_units - u0);
-#pragma unroll
-            for (int u = 0; u < B3_UPT; ++u) {
-                const uint32_t i = (uint32_t)u * B3_T + (uint32_t)tid;
-                v[u] = (i < nu) ? ldg_stream16(src + u0 + i) : make_uint4(0, 0, 0, 0);
-            }
-        }
-
-        // ---- the prefix (published long ago by now), row offsets, write-out ----
-        const unsigned long long excl = lookback_cta<false>(desc, tile, (uint32_t)total, lb_sum, lb_p);
-        if (tid == 0 && tile == n_tiles - 1) *nnz_out = (int64_t)(excl + (unsigned long long)total);
-        if (row_offsets) {
-#pragma unroll
-            for (int u = 0; u < B3_UPT; ++u) {
-                const uint32_t i = (uint32_t)u * B3_T + (uint32_t)tid;
-                if (i < nun) {
-                    const uint32_t gu = nu0 + i, r = fd_div(gu, upr);
-                    if (r * upr.d == gu) row_offsets[r] = (int64_t)(excl + (unsigned long long)off[u]);
-                }
-            }
-        }
-        run_to_global(values, excl, total, stage0);
-        if (!more) break;
-        tile = next;
-        __syncthreads();                                   // the staging buffer, mask_w and the look-back arrays are reused
-    }
-}
-
 // expansion: mask bytes -> counts -> scan -> look-back -> the tile's run of `values` into shared memory (aligned 16-byte loads, so that
 // run element j sits at stage element j + shift) -> dense tile, 16-byte stores
-__global__ void __launch_bounds__(B3_T) bitmask_expand_tile_kernel(const uint16_t* __restrict__ values, const uint8_t* __restrict__ bitmask,
-                                                                   uint4* __restrict__ dense, unsigned long long* __restrict__ desc,
-                                                                   uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles) {
-    __shared__ __align__(16) uint16_t stage[8 * B3_TILE + 16];
-    __shared__ uint32_t mask_s[B3_TILE / 4];
-    __shared__ int warp_tot[B3_UPT][B3_W];
-    __shared__ unsigned long long lb_sum[B3_W];
-    __shared__ int lb_p[B3_W];
+__global__ void __launch_bounds__(BM_THREADS) bitmask_expand_tile_kernel(const uint16_t* __restrict__ values, const uint8_t* __restrict__ bitmask,
+                                                                         uint4* __restrict__ dense, unsigned long long* __restrict__ desc,
+                                                                         uint32_t* __restrict__ ticket, uint32_t n_units, uint32_t n_tiles) {
+    __shared__ __align__(16) uint16_t stage[8 * BM_TILE + 16];
+    __shared__ uint32_t mask_s[BM_TILE / 4];
+    __shared__ int warp_tot[BM_UPT][BM_WARPS];
+    __shared__ unsigned long long lb_sum[BM_WARPS];
+    __shared__ int lb_p[BM_WARPS];
     __shared__ uint32_t tile_s;
     const int tid = threadIdx.x;
     if (tid == 0) tile_s = atomicAdd(ticket, 1u);
     __syncthreads();
     const uint32_t tile = tile_s;
-    const uint32_t u0 = tile * B3_TILE;
-    const uint32_t nu = min((uint32_t)B3_TILE, n_units - u0);
+    const uint32_t u0 = tile * BM_TILE;
+    const uint32_t nu = min((uint32_t)BM_TILE, n_units - u0);
     // the tile's mask bytes: 2 coalesced words per thread (n_units % 4 == 0)
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
-        const uint32_t wi = j * B3_T + tid;
+        const uint32_t wi = j * BM_THREADS + tid;
         mask_s[wi] = (wi * 4 < nu) ? __ldg(reinterpret_cast<const uint32_t*>(bitmask + u0) + wi) : 0u;
     }
     __syncthreads();
     uint32_t bytes_lo = 0, bytes_hi = 0;
-    int cnt[B3_UPT], off[B3_UPT];
+    int cnt[BM_UPT], off[BM_UPT];
 #pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) {
-        const uint32_t i = k * B3_T + tid;
+    for (int k = 0; k < BM_UPT; ++k) {
+        const uint32_t i = k * BM_THREADS + tid;
         const uint32_t b = (i < nu) ? reinterpret_cast<const uint8_t*>(mask_s)[i] : 0u;
         if (k < 4) bytes_lo |= b << (8 * k);
         else bytes_hi |= b << (8 * (k - 4));
@@ -1096,7 +415,7 @@ __global__ void __launch_bounds__(B3_T) bitmask_expand_tile_kernel(const uint16_
     const uint32_t nvec = (shift + (uint32_t)total + 7) >> 3;
     const uint4* gv = reinterpret_cast<const uint4*>(values + (excl - shift));
     const uint32_t span = shift + (uint32_t)total;
-    for (uint32_t c = tid; c < nvec; c += B3_T) {
+    for (uint32_t c = tid; c < nvec; c += BM_THREADS) {
         if (8 * c + 8 <= span) reinterpret_cast<uint4*>(stage)[c] = ldg_stream16(gv + c);    // c == 0 may include up to 7 elements of the previous tile's run
         else {
             for (uint32_t pos = 8 * c; pos < span; ++pos) stage[pos] = values[excl - shift + pos];   // the last vector: never read past the run (= past `values`)
@@ -1104,8 +423,8 @@ __global__ void __launch_bounds__(B3_T) bitmask_expand_tile_kernel(const uint16_
     }
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < B3_UPT; ++k) {
-        const uint32_t i = k * B3_T + tid;
+    for (int k = 0; k < BM_UPT; ++k) {
+        const uint32_t i = k * BM_THREADS + tid;
         if (i < nu) {
             const uint32_t b = (k < 4 ? bytes_lo >> (8 * k) : bytes_hi >> (8 * (k - 4))) & 0xffu;
             uint32_t e[8];
@@ -1128,54 +447,22 @@ template <bool COMPRESS>
 int launch_bitmask_lookback(const void* src, uint8_t* bitmask, void* dst, int64_t* row_offsets, int64_t* nnz_out, int64_t rows, int64_t cols,
                             int device, cudaStream_t st) {
     const int64_t n_units = rows * cols / 8;
-    const bool v1 = getenv("CT_B200_BITMASK_V1") != nullptr;
-    const int64_t tile_units = v1 ? BM_TILE : B3_TILE;
-    const uint32_t n_tiles = (uint32_t)((n_units + tile_units - 1) / tile_units);
+    const uint32_t n_tiles = (uint32_t)((n_units + BM_TILE - 1) / BM_TILE);
     uint8_t* scratch = nullptr;
     const size_t bytes = 16 + (size_t)n_tiles * sizeof(unsigned long long);
     int rc = scratch_alloc(reinterpret_cast<void**>(&scratch), bytes, device, st);
     if (rc) return rc;
     CT_CUDA_TRY(cudaMemsetAsync(scratch, 0, bytes, st));
-    if (!v1) {
-        if (COMPRESS && getenv("CT_B200_BITMASK_V6")) {       // the register-tile scatter experiment: slower than v5, kept for the record
-            CT_CUDA_TRY(cudaFuncSetAttribute(bitmask_compress_regs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B6_SMEM));
-            int occ = 0;
-            CT_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, bitmask_compress_regs_kernel, B3_T, B6_SMEM));
-            uint32_t grid = (uint32_t)(occ > 0 ? occ : 1) * (uint32_t)sm_count(device);
-            if (const char* e = getenv("CT_B200_BITMASK_GRID")) grid = (uint32_t)atoi(e);    // measurement aid
-            if (grid > n_tiles) grid = n_tiles;
-            if (grid < 1) grid = 1;
-            bitmask_compress_regs_kernel<<<grid, B3_T, B6_SMEM, st>>>(reinterpret_cast<const uint4*>(src), bitmask, reinterpret_cast<uint16_t*>(dst),
-                                                                          row_offsets, nnz_out, reinterpret_cast<unsigned long long*>(scratch + 16),
-                                                                          reinterpret_cast<uint32_t*>(scratch), (uint32_t)n_units, n_tiles,
-                                                                          make_fastdiv((uint64_t)(cols / 8)));
-        } else if (COMPRESS && !getenv("CT_B200_BITMASK_V3") && !getenv("CT_B200_BITMASK_V4")) {
-            CT_CUDA_TRY(cudaFuncSetAttribute(bitmask_compress_late_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B5_SMEM));
-            bitmask_compress_late_kernel<<<n_tiles, B3_T, B5_SMEM, st>>>(reinterpret_cast<const uint8_t*>(src), bitmask, reinterpret_cast<uint16_t*>(dst),
-                                                                          row_offsets, nnz_out, reinterpret_cast<unsigned long long*>(scratch + 16),
-                                                                          reinterpret_cast<uint32_t*>(scratch), (uint32_t)n_units, n_tiles,
-                                                                          make_fastdiv((uint64_t)(cols / 8)));
-        } else if (COMPRESS && !getenv("CT_B200_BITMASK_V3")) {
-            CT_CUDA_TRY(cudaFuncSetAttribute(bitmask_compress_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B4_SMEM));
-            bitmask_compress_gather_kernel<<<n_tiles, B3_T, B4_SMEM, st>>>(reinterpret_cast<const uint8_t*>(src), bitmask, reinterpret_cast<uint16_t*>(dst),
-                                                                            row_offsets, nnz_out, reinterpret_cast<unsigned long long*>(scratch + 16),
-                                                                            reinterpret_cast<uint32_t*>(scratch), (uint32_t)n_units, n_tiles,
-                                                                            make_fastdiv((uint64_t)(cols / 8)));
-        } else if (COMPRESS) {
-            auto kfn = bitmask_compress_tile_kernel;
-            CT_CUDA_TRY(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B3_SMEM));
-            kfn<<<n_tiles, B3_T, B3_SMEM, st>>>(reinterpret_cast<const uint8_t*>(src), bitmask, reinterpret_cast<uint16_t*>(dst), row_offsets, nnz_out,
-                                                reinterpret_cast<unsigned long long*>(scratch + 16), reinterpret_cast<uint32_t*>(scratch),
-                                                (uint32_t)n_units, n_tiles, make_fastdiv((uint64_t)(cols / 8)));
-        } else {
-            bitmask_expand_tile_kernel<<<n_tiles, B3_T, 0, st>>>(reinterpret_cast<const uint16_t*>(src), bitmask, reinterpret_cast<uint4*>(dst),
-                                                                 reinterpret_cast<unsigned long long*>(scratch + 16), reinterpret_cast<uint32_t*>(scratch),
-                                                                 (uint32_t)n_units, n_tiles);
-        }
+    unsigned long long* desc = reinterpret_cast<unsigned long long*>(scratch + 16);
+    uint32_t* ticket = reinterpret_cast<uint32_t*>(scratch);
+    if (COMPRESS) {
+        CT_CUDA_TRY(cudaFuncSetAttribute(bitmask_compress_late_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BM_SMEM));
+        bitmask_compress_late_kernel<<<n_tiles, BM_THREADS, BM_SMEM, st>>>(reinterpret_cast<const uint8_t*>(src), bitmask, reinterpret_cast<uint16_t*>(dst),
+                                                                           row_offsets, nnz_out, desc, ticket, (uint32_t)n_units, n_tiles,
+                                                                           make_fastdiv((uint64_t)(cols / 8)));
     } else {
-        bitmask_lookback_kernel<COMPRESS><<<n_tiles, 256, 0, st>>>(src, bitmask, dst, row_offsets, nnz_out,
-                                                                   reinterpret_cast<unsigned long long*>(scratch + 16), reinterpret_cast<uint32_t*>(scratch),
-                                                                   (uint32_t)n_units, n_tiles, make_fastdiv((uint64_t)(cols / 8)));
+        bitmask_expand_tile_kernel<<<n_tiles, BM_THREADS, 0, st>>>(reinterpret_cast<const uint16_t*>(src), bitmask, reinterpret_cast<uint4*>(dst),
+                                                                   desc, ticket, (uint32_t)n_units, n_tiles);
     }
     count_launch();
     cudaFreeAsync(scratch, st);

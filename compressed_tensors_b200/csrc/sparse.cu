@@ -670,7 +670,7 @@ __global__ void __launch_bounds__(EXR_THREADS, (U <= 4 ? 6 : 4)) bitmask_expand_
 }
 
 static bool bitmask_expand_rows_ok(int64_t rows, int units, const void* values) {
-    return rows >= 2 && units % 16 == 0 && units <= 2048 && aligned16(values) && !getenv("CT_B200_BITMASK_ROWS_V1");
+    return rows >= 2 && units % 16 == 0 && units <= 2048 && aligned16(values);
 }
 
 template <int U>
@@ -679,7 +679,8 @@ static int launch_bitmask_expand_rows_u(const void* values, const uint8_t* bitma
     const uint32_t vcap = (uint32_t)units * 16u + 32u;
     const uint32_t worst = vcap + (uint32_t)units;                 // an entry of a full row
     int pct = 150;                                                 // ring = 1.5 worst-case rows
-    if (const char* e = getenv("CT_B200_BITMASK_RING_PCT")) pct = atoi(e);   // measurement aid
+    // test hook: at 100 % the ring holds exactly one worst-case row, a case no input reaches otherwise
+    if (const char* e = getenv("CT_B200_BITMASK_RING_PCT")) pct = atoi(e);
     if (pct < 100) pct = 100;
     if (pct > 600) pct = 600;
     const uint32_t ring = (uint32_t)((uint64_t)worst * pct / 100 + 15) / 16 * 16;
@@ -708,8 +709,7 @@ static int launch_bitmask_expand_rows(const void* values, const uint8_t* bitmask
 // rows shorter than one 4-segment iteration keep the single-segment shape (less shared memory, more blocks per SM)
 template <bool COMPRESS>
 static void launch_bitmask_move_vec16(const void* src, const uint8_t* bitmask, const int64_t* row_offsets, void* dst, int64_t rows, int units, cudaStream_t st) {
-    int cap = COMPRESS ? 2 : 4;   // compress keeps its 16-byte loads in registers: 4 segments cost 79 registers (3 blocks per SM)
-    if (const char* e = getenv("CT_B200_BITMASK_SEGMENTS")) cap = atoi(e);   // measurement aid (tools/jitter.py)
+    const int cap = COMPRESS ? 2 : 4;   // compress keeps its 16-byte loads in registers: 4 segments cost 79 registers (3 blocks per SM)
     if (units > 512 && cap >= 4) bitmask_move_vec16_kernel<COMPRESS, 4><<<(unsigned)rows, 256, 0, st>>>(src, bitmask, row_offsets, dst, units);
     else if (units > 256 && cap >= 2) bitmask_move_vec16_kernel<COMPRESS, 2><<<(unsigned)rows, 256, 0, st>>>(src, bitmask, row_offsets, dst, units);
     else bitmask_move_vec16_kernel<COMPRESS, 1><<<(unsigned)rows, 256, 0, st>>>(src, bitmask, row_offsets, dst, units);
@@ -889,7 +889,7 @@ int ct_bitmask_compress_onepass(const void* x, int dtype, void* values, uint8_t*
         return CT_OK;
     }
     if (!x || !values || !bitmask) { set_error("null pointer"); return CT_E_ARG; }
-    if (bitmask_lookback_ok(dtype, rows, cols, x, bitmask, values) && !getenv("CT_B200_BITMASK_TWO_PHASE"))
+    if (bitmask_lookback_ok(dtype, rows, cols, x, bitmask, values))
         return launch_bitmask_lookback<true>(x, bitmask, values, row_offsets, nnz_out, rows, cols, device, st);
     // every other dtype / shape: the two-phase kernels with a stream-ordered workspace (still no host synchronisation)
     void* ws = nullptr;
@@ -909,10 +909,9 @@ int ct_bitmask_decompress(const void* values, int dtype, const uint8_t* bitmask,
     const int64_t nb = (cols + 7) / 8;
     const unsigned g = (unsigned)(rows < GRID_SMS * 8 ? rows : GRID_SMS * 8);
     // With the format's row_offsets the expansion is ONE pass already (every row knows where its values start): the pipelined row
-    // kernel, or the per-row kernel for shapes it declines.  The
-    // look-back kernel (flat tiles, the scan recomputed from the mask popcounts, slower) serves callers that do not have
-    // row_offsets, and CT_B200_BITMASK_LOOKBACK=1 for measurements.
-    if (values && (!row_offsets || getenv("CT_B200_BITMASK_LOOKBACK")) && bitmask_lookback_ok(dtype, rows, cols, out, bitmask, values))
+    // kernel, or the per-row kernel for shapes it declines.  The look-back kernel (flat tiles, the scan recomputed from the mask
+    // popcounts, slower) serves callers that do not have row_offsets.
+    if (values && !row_offsets && bitmask_lookback_ok(dtype, rows, cols, out, bitmask, values))
         return launch_bitmask_lookback<false>(values, const_cast<uint8_t*>(bitmask), out, nullptr, nullptr, rows, cols, device, st);
     if (!row_offsets) { set_error("bitmask_decompress without row_offsets needs a 2-byte dtype, cols %% 8 == 0 and aligned tensors"); return CT_E_UNSUPPORTED; }
     if (bitmask_vec16_ok(dtype, rows, cols, out, bitmask) && (reinterpret_cast<uintptr_t>(bitmask) & 15u) == 0 &&

@@ -463,12 +463,13 @@ def test_bitmask_compress_vs_oracle(dtype, shape):
     same(dense.cpu(), x.where(x != 0, torch.zeros_like(x)), "")
 
 
-@pytest.mark.parametrize("shape", [(2, 128), (5, 16384), (3, 16512), (1, 8192), (37, 8192), (700, 4096), (150, 14336)])
+@pytest.mark.parametrize("shape", [(2, 128), (5, 16384), (3, 16512), (1, 8192), (37, 8192), (700, 4096), (150, 14336),
+                                   (37, 4128), (5, 2080), (9, 1056)])
 def test_bitmask_expand_rows_pipeline(shape, monkeypatch):
-    """the pipelined row expansion (persistent CTAs, bulk-copy ring; csrc/sparse.cu bitmask_expand_rows_kernel) against the oracle and
-    against the per-row kernel it replaces: rows that are empty, full, and mixed; more rows than one CTA's ring holds; the last rows of
-    the tensor (values fetched after the scan, because the run's 16-byte over-read would leave `values`); shapes the pipeline declines
-    (one row, more than 2048 units per row)"""
+    """the pipelined row expansion (persistent CTAs, bulk-copy ring; csrc/sparse.cu bitmask_expand_rows_kernel) against the oracle:
+    rows that are empty, full, and mixed; more rows than one CTA's ring holds; the last rows of the tensor (values fetched after the
+    scan, because the run's 16-byte over-read would leave `values`); and the per-row kernel on the shapes the pipeline declines (one
+    row, more than 2048 units per row, cols % 128 != 0 with 4, 2 and 1 segments per iteration)"""
     g = torch.Generator().manual_seed(shape[0] * 7 + shape[1])
     x = (torch.randn(shape, generator=g) * 3).bfloat16()
     x[torch.rand(shape, generator=g) < 0.5] = 0
@@ -484,10 +485,7 @@ def test_bitmask_expand_rows_pipeline(shape, monkeypatch):
     launches = N.launch_count()
     dense = ops.bitmask_decompress(gv, gb, go, x.shape)
     assert N.launch_count() - launches == 1
-    same(dense.cpu(), want, "pipelined expand vs oracle")
-    monkeypatch.setenv("CT_B200_BITMASK_ROWS_V1", "1")
-    same(ops.bitmask_decompress(gv, gb, go, x.shape), dense, "per-row kernel == pipelined kernel")
-    monkeypatch.delenv("CT_B200_BITMASK_ROWS_V1")
+    same(dense.cpu(), want, "row expand vs oracle")
     for pct in ("100", "400"):                              # ring of exactly one worst-case row (no prefetch at full density) / a deep one
         monkeypatch.setenv("CT_B200_BITMASK_RING_PCT", pct)
         same(ops.bitmask_decompress(gv, gb, go, x.shape), dense, f"ring {pct} %")
@@ -495,10 +493,11 @@ def test_bitmask_expand_rows_pipeline(shape, monkeypatch):
 
 @pytest.mark.parametrize("density", [0.0, 0.03, 0.5, 0.97, 1.0])
 @pytest.mark.parametrize("shape", [(8, 32), (64, 4096), (300, 1000), (1031, 2056), (4096, 14336)])
-def test_bitmask_onepass_lookback_vs_oracle(shape, density, monkeypatch):
+def test_bitmask_onepass_lookback_vs_oracle(shape, density):
     """the one-pass kernels (decoupled look-back scan, csrc/bitmask_onepass.cu): every output of the format -- values, mask bytes,
     row offsets, nnz -- against the restated oracle, the no-sync (`exact=False`) form included, for densities from empty to full, tiles
-    that hold many rows and rows that span many tiles; and the same bits as the two-phase kernels they replace"""
+    that hold many rows and rows that span many tiles; the same bits as the two-phase ABI (count -> scan -> move); and the expansion
+    without row_offsets, which recomputes the scan from the mask popcounts"""
     g = torch.Generator().manual_seed(shape[1] + int(density * 100))
     x = (torch.randn(shape, generator=g) * 3).bfloat16()
     x[torch.rand(shape, generator=g) >= density] = 0
@@ -521,8 +520,20 @@ def test_bitmask_onepass_lookback_vs_oracle(shape, density, monkeypatch):
     assert N.launch_count() - launches == 1
     same(dense.cpu(), x.where(x != 0, torch.zeros_like(x)), "expand")
     same(dense.cpu(), oracle.bitmask_decompress(vals, bm, x.shape), "expand vs oracle")
-    monkeypatch.setenv("CT_B200_BITMASK_TWO_PHASE", "1")     # count -> scan -> move
-    tv, tb, to = ops.bitmask_compress(xd)
+    rows, cols = shape
+    st = N.stream_ptr(0)
+    tb = torch.empty_like(gb)
+    to = torch.empty_like(go)
+    tn = torch.empty(1, dtype=torch.int64, device=DEV)
+    ws = torch.empty(N.lib().ct_bitmask_workspace_bytes(rows, cols), dtype=torch.uint8, device=DEV)
+    N.check(N.lib().ct_bitmask_count(N.ptr(xd), N.DT[x.dtype], N.ptr(tb), N.ptr(to), N.ptr(tn), N.ptr(ws), rows, cols, 0, st))
+    tv = torch.empty(int(tn.item()), dtype=x.dtype, device=DEV)
+    N.check(N.lib().ct_bitmask_compress(N.ptr(xd), N.DT[x.dtype], N.ptr(tb), N.ptr(to), N.ptr(tv), rows, cols, 0, st))
     same(tv, gv, "two-phase values"); same_values(tb, gb, "two-phase mask"); same_values(to, go, "two-phase offsets")
-    monkeypatch.setenv("CT_B200_BITMASK_LOOKBACK", "1")      # expansion without row_offsets: the scan recomputed from the mask popcounts
-    same(ops.bitmask_decompress(gv, gb, go, x.shape), dense, "look-back expand == row_offsets expand")
+    out = torch.empty_like(xd)
+    rc = N.lib().ct_bitmask_decompress(N.ptr(cap), N.DT[x.dtype], N.ptr(gb), N.ptr(None), N.ptr(out), rows, cols, 0, st)
+    if onepass:
+        N.check(rc)
+        same(out, dense, "look-back expand == row_offsets expand")
+    else:
+        assert rc == N.CT_E_UNSUPPORTED                      # without row_offsets only the look-back kernel can expand

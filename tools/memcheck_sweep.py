@@ -80,14 +80,10 @@ def sparse_family(rows, cols, dt):
     ops.bitmask_decompress(v, m, o, (rows, cols))
     b = torch.rand(rows, cols, device=DEV) < 0.3
     ops.unpack_bitmasks(ops.pack_bitmasks(b), (rows, cols))
-    # round 2: one-pass bitmask (ring kernel + look-back; also the v1 look-back kernel), fused 2:4 + int4
+    # round 2: one-pass bitmask (ring kernel + look-back), fused 2:4 + int4
     for density in (0.0, 0.07, 1.0):
         u = torch.where(torch.rand(rows, cols, device=DEV) < density, x, torch.zeros_like(x))
-        for v1 in (False, True):
-            if v1:
-                os.environ["CT_B200_BITMASK_V1"] = "1"
-            v, m, o, n = ops.bitmask_compress(u, exact=False)
-            os.environ.pop("CT_B200_BITMASK_V1", None)
+        v, m, o, n = ops.bitmask_compress(u, exact=False)
         ops.bitmask_decompress(v[: int(n.item())].clone(), m, o, (rows, cols))
     if cols % 4 == 0 and dt != torch.float32:
         for a, shape in ((qa(num_bits=4, type="int", strategy="channel"), (rows, 1)), (qa(num_bits=4, type="int", strategy="group", group_size=32), (rows, max(cols // 32, 1)))):
