@@ -455,8 +455,9 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
     for (int i = 0; i < n; ++i) {
         if (done[i]) continue;
         if (!plans[i].fast) {
+            // an empty tensor has nothing to compute, whatever op it is in (the fused-only ops would otherwise refuse it)
+            if (descs[i].rows * descs[i].cols == 0) { done[i] = 1; continue; }
             if (bits_op) {
-                if (descs[i].rows * descs[i].cols == 0) { done[i] = 1; continue; }
                 rc = (op == CT_OP_PACK_INT32)
                          ? launch_generic_pack(reinterpret_cast<const int8_t*>(in[i]), reinterpret_cast<int32_t*>(out[i]), descs[i].rows, descs[i].cols, descs[i].num_bits, 1, stream)
                          : launch_generic_unpack(reinterpret_cast<const int32_t*>(in[i]), reinterpret_cast<int8_t*>(out[i]), descs[i].rows, descs[i].cols, descs[i].num_bits, 1, stream);
