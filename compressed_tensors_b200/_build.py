@@ -83,29 +83,6 @@ def _compile(src: str, force: bool, verbose: bool) -> str:
     return obj
 
 
-def build_variant(tag: str, defines: list) -> str:
-    """an A/B variant of the library (e.g. another tile size) next to the shipped one: libct_b200_<tag>.so, objects in csrc/build_<tag>/;
-    selected at run time with CT_B200_LIB=<path> (compressed_tensors_b200/_native.py)"""
-    obj_dir = os.path.join(CSRC, f"build_{tag}")
-    os.makedirs(obj_dir, exist_ok=True)
-    lib = os.path.join(HERE, f"libct_b200_{tag}.so")
-
-    def one(src):
-        obj = os.path.join(obj_dir, src.replace(".cu", ".o"))
-        r = subprocess.run([nvcc(), *NVCC_FLAGS, *defines, "-c", os.path.join(CSRC, src), "-o", obj], capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
-        return obj
-
-    with cf.ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 4)) as ex:
-        objs = list(ex.map(one, SOURCES))
-    r = subprocess.run([nvcc(), "-shared", "-o", lib, *objs, *ARCH, "-Xcompiler", "-fPIC", "-Xcompiler", "-fopenmp"],
-                       capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
-    return lib
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJ, exist_ok=True)
     newest_src = max(max(os.path.getmtime(os.path.join(CSRC, s)) for s in SOURCES), _newest_header())
@@ -121,8 +98,4 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:       # python -m compressed_tensors_b200._build --variant t2048 -DCT_TILE_CHUNKS=2048
-        i = sys.argv.index("--variant")
-        print(build_variant(sys.argv[i + 1], sys.argv[i + 2:]))
-    else:
-        print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))

@@ -14,7 +14,8 @@ from typing import Optional
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("CT_B200_LIB") or os.path.join(_HERE, "libct_b200.so")   # CT_B200_LIB: an A/B build variant (_build.build_variant)
+# CT_B200_LIB loads another build of the library, for example the parent commit's, for A/B timing
+LIB_PATH = os.environ.get("CT_B200_LIB") or os.path.join(_HERE, "libct_b200.so")
 
 INF = (1 << 63) - 1  # CT_DIV_INF
 
@@ -83,7 +84,6 @@ _PROTOS = {
     "ct_last_error": (ctypes.c_char_p, []),
     "ct_device_count": (_int, []),
     "ct_device_ok": (_int, [_int]),
-    "ct_set_tuning": (_int, [_int, _int, _int]),
     "ct_launch_count": (_i64, []),
     "ct_pack_int32": (_int, [_vp, _vp, _i64, _i64, _int, _int, _int, _vp]),
     "ct_unpack_int32": (_int, [_vp, _vp, _i64, _i64, _int, _int, _int, _vp]),
@@ -189,6 +189,3 @@ def ptr(t: Optional[torch.Tensor]) -> ctypes.c_void_p:
 def launch_count() -> int:
     return int(lib().ct_launch_count())
 
-
-def set_tuning(pipe: int, stages: int = 4, ctas_per_sm: int = 0) -> None:
-    lib().ct_set_tuning(int(pipe), int(stages), int(ctas_per_sm))

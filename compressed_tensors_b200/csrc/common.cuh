@@ -24,15 +24,7 @@ void count_launch(int n = 1);
         if (_e != cudaSuccess) return ctb::cuda_fail(_e, #expr); \
     } while (0)
 
-struct Tuning {
-    int pipe;         // 0 direct loads, 1 TMA bulk ring
-    int stages;       // ring depth for the TMA variant
-    int ctas_per_sm;  // persistent CTAs per SM
-    int dynamic;      // TMA variant: 1 = tiles claimed from a device counter (default), 0 = static round-robin deal
-    int auto_shape;   // 1 when stages / ctas_per_sm are the defaults (not set by env / ct_set_tuning): ops may use their own preference
-};
 constexpr int DYNAMIC_MIN_TILES_PER_SM = 24;   // below this many tiles per SM a launch keeps the static deal (no scratch, no memset)
-Tuning tuning();
 constexpr int GRID_SMS = 132;   // SMs of an H100 SXM: grid size of the grid-stride kernels, sm_count() when the device is unknown
 int sm_count(int device);
 int64_t l2_bytes(int device);   // L2 cache size of the device (0 when unknown)
@@ -98,11 +90,6 @@ __device__ __forceinline__ uint4 ldg_stream16(const void* p) {
 __device__ __forceinline__ uint2 ldg_stream8(const void* p) {
     uint2 r;
     asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-    return r;
-}
-__device__ __forceinline__ uint32_t ldg_stream4(const void* p) {
-    uint32_t r;
-    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
     return r;
 }
 __device__ __forceinline__ void stg_stream16(void* p, const uint4& v) {

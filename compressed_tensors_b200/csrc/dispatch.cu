@@ -496,7 +496,7 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
         // Launches with few tiles per CTA keep the static deal and need no scratch at all.
         uint8_t* scratch = nullptr;
         const bool many = jobs.size() > 1;
-        const bool dynamic = tuning().dynamic && (uint64_t)tiles * tc >= (uint64_t)DYNAMIC_MIN_TILES_PER_SM * TILE_CHUNKS * sm_count(device);
+        const bool dynamic = (uint64_t)tiles * tc >= (uint64_t)DYNAMIC_MIN_TILES_PER_SM * TILE_CHUNKS * sm_count(device);
         if (many || dynamic) {
             const size_t tbl_bytes = many ? jobs.size() * sizeof(Job) : 0;
             rc = scratch_alloc(reinterpret_cast<void**>(&scratch), 16 + tbl_bytes, device, stream);

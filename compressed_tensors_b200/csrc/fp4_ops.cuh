@@ -366,7 +366,7 @@ template <class P, int SK>
 struct Fp4UnpackDequantOp {
     static constexpr int IN_BYTES = 4;
     static constexpr int GROUP = 1;
-    // launch shape: the default (4 stages x 3 CTAs per SM; tools/jitter.py --tune compares others)
+    // launch shape: the default ring, 4 stages x 3 CTAs per SM (stream.cuh: ring_shape)
     using Raw = Fp4DqRaw;
     __device__ static __forceinline__ Raw prefetch(const Job& J, uint32_t gc0) {
         Raw r;

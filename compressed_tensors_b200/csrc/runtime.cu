@@ -1,9 +1,7 @@
-// runtime.cu -- error strings, device checks, tuning knobs, launch counter.
+// runtime.cu -- error strings, device checks, launch counter.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
-#include <cstring>
 #include <mutex>
 
 #include "engine.h"
@@ -27,41 +25,6 @@ int cuda_fail(cudaError_t e, const char* what) {
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
-
-// ---- tuning ---------------------------------------------------------------------------------
-static std::mutex g_tune_mu;
-static Tuning g_tune = {-1, 0, 0, 1, 0};
-
-static int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    if (!v || !*v) return dflt;
-    if (!strcmp(v, "tma")) return 1;
-    if (!strcmp(v, "tma-static")) return 2;
-    if (!strcmp(v, "direct")) return 0;
-    return atoi(v);
-}
-
-Tuning tuning() {
-    std::lock_guard<std::mutex> lk(g_tune_mu);
-    if (g_tune.pipe < 0) {
-        const int p = env_int("CT_B200_PIPE", 1);
-        g_tune.pipe = p ? 1 : 0;
-        g_tune.dynamic = p == 2 ? 0 : 1;
-        g_tune.stages = env_int("CT_B200_STAGES", 4);
-        g_tune.ctas_per_sm = env_int("CT_B200_CTAS_PER_SM", 0);
-    }
-    Tuning t = g_tune;
-    t.auto_shape = (t.ctas_per_sm <= 0) ? 1 : 0;
-    if (t.ctas_per_sm <= 0) t.ctas_per_sm = (t.pipe == 1) ? 3 : 8;
-    return t;
-}
-void set_tuning(int pipe, int stages, int ctas) {
-    std::lock_guard<std::mutex> lk(g_tune_mu);
-    g_tune.pipe = pipe ? 1 : 0;
-    g_tune.dynamic = pipe == 2 ? 0 : 1;
-    g_tune.stages = stages > 0 ? stages : 4;
-    g_tune.ctas_per_sm = ctas;
-}
 
 // ---- devices --------------------------------------------------------------------------------
 static std::mutex g_dev_mu;
@@ -143,9 +106,5 @@ int ct_device_count(void) {
     return n;
 }
 int ct_device_ok(int device) { return ctb::check_device(device) == CT_OK ? 1 : 0; }
-int ct_set_tuning(int pipe, int stages, int ctas_per_sm) {
-    ctb::set_tuning(pipe, stages, ctas_per_sm);
-    return CT_OK;
-}
 int64_t ct_launch_count(void) { return ctb::launch_count(); }
 }

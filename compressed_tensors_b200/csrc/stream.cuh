@@ -1,4 +1,4 @@
-// stream.cuh -- the two persistent streaming pipelines every hot-path op is instantiated on.
+// stream.cuh -- the persistent streaming pipeline every hot-path op is instantiated on.
 //
 // Work decomposition (all hot-path ops are elementwise over a flat, contiguous tensor):
 //   chunk = 8 consecutive elements
@@ -10,36 +10,26 @@
 //           globally and CLAIMED from a device counter by a persistent grid of n_SM * ctas_per_sm CTAs
 //           (dynamic schedule, see stream_tma_kernel; small launches keep a static round-robin deal).
 //
-// Pipeline 1 ("tma"): warp-specialised.  One producer lane issues 1-D bulk async copies
+// The pipeline is warp-specialised.  One producer lane issues 1-D bulk async copies
 // (cp.async.bulk, the TMA engine without a tensor map) of whole input tiles into a ring of
 // shared-memory stages, each guarded by a full/empty mbarrier pair (waits use the hardware
 // suspend hint, so the idle producer does not burn issue slots).  NCW consumer warps wait on the
 // full barrier, read their units from shared memory with bank-conflict-free swizzled LDS.128, do
 // the arithmetic in registers and write with coalesced 16-byte streaming stores.  The scale loads
 // of a tile are issued BEFORE the barrier wait and consumed after it.
-// Pipeline 0 ("direct"): every thread issues its tile's 128-bit global loads up front and relies on
-// occupancy for memory-level parallelism (kept as the comparison point and for profiling).
 #pragma once
 
 #include "common.cuh"
 
 namespace ctb {
 
-#ifndef CT_TILE_CHUNKS
-#define CT_TILE_CHUNKS 1024
-#endif
-constexpr int TILE_CHUNKS = CT_TILE_CHUNKS;   // default tile: 1024 chunks = 8192 elements (16 KB of bf16); build-time knob for A/B variants
-#ifndef CT_BIG_TILE_CHUNKS
-#define CT_BIG_TILE_CHUNKS 2048
-#endif
+constexpr int TILE_CHUNKS = 1024;   // default tile: 1024 chunks = 8192 elements (16 KB of bf16)
 // An op may ask for another tile size (`static constexpr int TILE`).  The four headline 16-bit ops run on 2048-chunk tiles with a
-// 3-stage x 2-CTA ring: half the per-tile bookkeeping of the consumer warps for the same bytes in flight (the CT_BIG_TILE_CHUNKS
-// build knob and tools/jitter.py compare tile sizes).  The host side must count tiles with the
-// same number: sig_tile_chunks() in engine.h, checked at every launch.
-constexpr int BIG_TILE_CHUNKS = CT_BIG_TILE_CHUNKS;
+// 3-stage x 2-CTA ring: half the per-tile bookkeeping of the consumer warps for the same bytes in flight.  The host side must
+// count tiles with the same number: sig_tile_chunks() in engine.h, checked at every launch.
+constexpr int BIG_TILE_CHUNKS = 2048;
 constexpr int CHUNK_ELEMS = 8;
-constexpr int NCW = 8;              // consumer warps (tma pipeline)
-constexpr int DIRECT_THREADS = 256;
+constexpr int NCW = 8;              // consumer warps
 constexpr int MAX_STAGES = 12;
 
 struct Job {
@@ -94,8 +84,6 @@ __device__ __forceinline__ Job job_at(const JobTable& t, int j) {
 
 template <class Op, class = void> struct HasTile { static constexpr bool value = false; };
 template <class Op> struct HasTile<Op, decltype((void)sizeof(typename Op::Tile))> { static constexpr bool value = true; };
-template <class Op, class = void> struct HasShape { static constexpr bool value = false; };
-template <class Op> struct HasShape<Op, decltype((void)Op::PREF_CTAS)> { static constexpr bool value = true; };
 template <class Op, class = void> struct TileOf { static constexpr int value = TILE_CHUNKS; };
 template <class Op> struct TileOf<Op, decltype((void)Op::TILE)> { static constexpr int value = Op::TILE; };
 struct NoTile {};
@@ -120,24 +108,6 @@ __device__ __forceinline__ void lds_chunk(uint32_t saddr, uint32_t (&w)[BYTES / 
     } else {
         asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "r"(saddr));
         asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "r"(saddr + 16));
-    }
-}
-// CACHED = true keeps the line in L1 (several loads of one thread share 128-byte lines)
-template <int BYTES, bool CACHED>
-__device__ __forceinline__ void ldg_chunk(const uint8_t* p, uint32_t (&w)[BYTES / 4]) {
-    if constexpr (BYTES == 4) {
-        w[0] = CACHED ? __ldg(reinterpret_cast<const uint32_t*>(p)) : ldg_stream4(p);
-    } else if constexpr (BYTES == 8) {
-        uint2 v = CACHED ? __ldg(reinterpret_cast<const uint2*>(p)) : ldg_stream8(p);
-        w[0] = v.x; w[1] = v.y;
-    } else if constexpr (BYTES == 16) {
-        uint4 v = CACHED ? __ldg(reinterpret_cast<const uint4*>(p)) : ldg_stream16(p);
-        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
-    } else {
-        uint4 v = CACHED ? __ldg(reinterpret_cast<const uint4*>(p)) : ldg_stream16(p);
-        uint4 u = CACHED ? __ldg(reinterpret_cast<const uint4*>(p + 16)) : ldg_stream16(p + 16);
-        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
-        w[4] = u.x; w[5] = u.y; w[6] = u.z; w[7] = u.w;
     }
 }
 
@@ -179,12 +149,12 @@ __device__ __forceinline__ void rotate_out(uint32_t (&o)[GROUP * WPC], int off) 
 }
 
 // ------------------------------------------------------------------------------------
-// pipeline 1: TMA bulk-copy ring
+// TMA bulk-copy ring
 // ------------------------------------------------------------------------------------
 // Tile schedule.  `sched` != nullptr: DYNAMIC -- the producer lane of every CTA claims tile ids from a
 // zero-initialised device counter with atomicAdd, one claim in flight ahead of its use.  A static
 // round-robin deal makes the launch wait for the slowest SM: SMs do not all see the same memory
-// bandwidth, so equal shares finish at different times (tools/ubench/mix_ceiling.cu compares the two).  `sched` == nullptr: static deal (small launches, <= 1 tile a CTA).
+// bandwidth, so equal shares finish at different times (tools/ubench/mix_ceiling.cu compares the two).  `sched` == nullptr: static deal (launches of fewer than DYNAMIC_MIN_TILES_PER_SM tiles per SM, dispatch.cu).
 // Either way the producer publishes {tile, next tile} of a stage in shared memory before it arms the
 // stage's full barrier; consumers pick both up after the wait (release/acquire through the mbarrier).
 constexpr uint32_t SMEM_HDR = 384;   // full[12] | empty[12] | ids[12] (8 bytes each), then the data ring
@@ -340,46 +310,6 @@ __global__ void __launch_bounds__(32 * (NCW + 1)) stream_tma_kernel(const __grid
 }
 
 // ------------------------------------------------------------------------------------
-// pipeline 0: direct global loads
-// ------------------------------------------------------------------------------------
-template <class Op>
-__global__ void __launch_bounds__(DIRECT_THREADS) stream_direct_kernel(const __grid_constant__ JobTable tbl,
-                                                                       const __grid_constant__ Common cm,
-                                                                       uint32_t total_tiles) {
-    constexpr int TILE_CHUNKS = TileOf<Op>::value;
-    constexpr int G = Op::GROUP;
-    constexpr int UNITS = TILE_CHUNKS / G;
-    constexpr int ITERS = UNITS / DIRECT_THREADS;
-    int j = 0;
-    Job J = job_at(tbl, 0);
-    for (uint32_t tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        if (tile >= J.tile_end) {
-            while (tile >= job_tile_end(tbl, j)) ++j;
-            J = job_at(tbl, j);
-        }
-        const uint32_t base = (tile - J.tile_begin) * TILE_CHUNKS;
-        const uint32_t chunks = min((uint32_t)TILE_CHUNKS, J.n_chunks - base);
-        uint32_t w[ITERS][G][Op::IN_BYTES / 4];
-        typename Op::Raw raw[ITERS];
-#pragma unroll
-        for (int it = 0; it < ITERS; ++it) {
-            const uint32_t c0 = (uint32_t)(it * DIRECT_THREADS + threadIdx.x) * G;
-            if (c0 < chunks) {
-#pragma unroll
-                for (int k = 0; k < G; ++k) ldg_chunk<Op::IN_BYTES, (G > 1)>(J.in + (size_t)(base + c0 + k) * Op::IN_BYTES, w[it][k]);
-                raw[it] = Op::prefetch(J, base + c0);
-            }
-        }
-        const auto tc = op_tile<Op>(J);
-#pragma unroll
-        for (int it = 0; it < ITERS; ++it) {
-            const uint32_t c0 = (uint32_t)(it * DIRECT_THREADS + threadIdx.x) * G;
-            if (c0 < chunks) op_run<Op>(J, cm, raw[it], base + c0, w[it], 0, tc);
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------
 // host-side launcher shared by all ops
 // ------------------------------------------------------------------------------------
 struct LaunchPlan {
@@ -390,6 +320,26 @@ struct LaunchPlan {
     uint32_t* sched = nullptr;   // zeroed device counter for the dynamic tile schedule (nullptr = static deal); owned by dispatch.cu
 };
 
+// Ring shape of an op: its measured preference (`static constexpr int PREF_STAGES, PREF_CTAS`), 4 stages x 3 CTAs per SM for ops
+// that declare none, cut to fit: stages in [2, MAX_STAGES], then stages and after them CTAs reduced until stages * tile * ctas
+// stays within ~200 KB of shared memory per SM.
+struct RingShape {
+    int stages, ctas;
+};
+template <class Op, class = void> struct PrefRing { static constexpr RingShape value{4, 3}; };
+template <class Op> struct PrefRing<Op, decltype((void)Op::PREF_CTAS)> { static constexpr RingShape value{Op::PREF_STAGES, Op::PREF_CTAS}; };
+constexpr bool ring_fits(RingShape r, size_t tile_bytes) { return (size_t)r.stages * tile_bytes * r.ctas + 1024 * r.ctas <= 200 * 1024; }
+template <class Op>
+constexpr RingShape ring_shape() {
+    constexpr size_t TILE_BYTES = (size_t)TileOf<Op>::value * Op::IN_BYTES;
+    RingShape r = PrefRing<Op>::value;
+    if (r.stages < 2) r.stages = 2;
+    if (r.stages > MAX_STAGES) r.stages = MAX_STAGES;
+    while (!ring_fits(r, TILE_BYTES) && r.stages > 2) --r.stages;
+    while (!ring_fits(r, TILE_BYTES) && r.ctas > 1) --r.ctas;
+    return r;
+}
+
 template <class Op>
 int launch_stream(const LaunchPlan& lp, int device, cudaStream_t stream) {
     if (lp.total_tiles == 0) return CT_OK;
@@ -397,32 +347,15 @@ int launch_stream(const LaunchPlan& lp, int device, cudaStream_t stream) {
         set_error("internal: tiles counted with %d chunks, the kernel uses %d", lp.tile_chunks, TileOf<Op>::value);
         return CT_E_ARG;
     }
-    const Tuning tn = tuning();
-    const int sms = sm_count(device);
-    if (tn.pipe == 1) {
-        constexpr int TILE_BYTES = TileOf<Op>::value * Op::IN_BYTES;
-        int stages = tn.stages;
-        int ctas = tn.ctas_per_sm;
-        if constexpr (HasShape<Op>::value) {   // an op's measured preference, unless the caller tuned explicitly
-            if (tn.auto_shape) { stages = Op::PREF_STAGES; ctas = Op::PREF_CTAS; }
-        }
-        if (stages < 2) stages = 2;
-        if (stages > MAX_STAGES) stages = MAX_STAGES;
-        // keep stages * tile * ctas within ~200 KB of shared memory per SM
-        while ((size_t)stages * TILE_BYTES * ctas + 1024 * ctas > 200 * 1024 && stages > 2) --stages;
-        while ((size_t)stages * TILE_BYTES * ctas + 1024 * ctas > 200 * 1024 && ctas > 1) --ctas;
-        const size_t smem = SMEM_HDR + (size_t)stages * TILE_BYTES;
-        auto kfn = stream_tma_kernel<Op>;
-        CT_CUDA_TRY(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        uint32_t grid = (uint32_t)(sms * ctas);
-        if (grid > lp.total_tiles) grid = lp.total_tiles;
-        kfn<<<grid, 32 * (NCW + 1), smem, stream>>>(lp.tbl, lp.cm, lp.total_tiles, stages, grid < lp.total_tiles ? lp.sched : nullptr);
-    } else {
-        int ctas = tn.ctas_per_sm > 0 ? tn.ctas_per_sm : 8;
-        uint32_t grid = (uint32_t)(sms * ctas);
-        if (grid > lp.total_tiles) grid = lp.total_tiles;
-        stream_direct_kernel<Op><<<grid, DIRECT_THREADS, 0, stream>>>(lp.tbl, lp.cm, lp.total_tiles);
-    }
+    constexpr size_t TILE_BYTES = (size_t)TileOf<Op>::value * Op::IN_BYTES;
+    constexpr RingShape ring = ring_shape<Op>();
+    static_assert(ring_fits(ring, TILE_BYTES), "the op's tile does not fit a ring in 200 KB of shared memory");
+    constexpr size_t smem = SMEM_HDR + (size_t)ring.stages * TILE_BYTES;
+    auto kfn = stream_tma_kernel<Op>;
+    CT_CUDA_TRY(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    uint32_t grid = (uint32_t)(sm_count(device) * ring.ctas);
+    if (grid > lp.total_tiles) grid = lp.total_tiles;
+    kfn<<<grid, 32 * (NCW + 1), smem, stream>>>(lp.tbl, lp.cm, lp.total_tiles, ring.stages, grid < lp.total_tiles ? lp.sched : nullptr);
     count_launch();
     CT_CUDA_TRY(cudaGetLastError());
     return CT_OK;

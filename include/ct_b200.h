@@ -106,9 +106,6 @@ const char* ct_version(void);
 const char* ct_last_error(void);
 int ct_device_count(void);                 /* 0 when no CUDA device / driver */
 int ct_device_ok(int device);              /* 1 if `device` is sm_90 (H100) */
-/* tuning knobs (also read from env CT_B200_PIPE / CT_B200_STAGES / CT_B200_CTAS_PER_SM):
- * pipe 0 = direct 128-bit global loads, 1 = TMA bulk-copy shared-memory ring with dynamic tile claims, 2 = same ring, static deal */
-int ct_set_tuning(int pipe, int stages, int ctas_per_sm);
 /* number of kernels this library has launched in the calling process */
 int64_t ct_launch_count(void);
 

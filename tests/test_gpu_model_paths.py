@@ -3,7 +3,7 @@ The paths a whole model takes, element by element against the CPU oracle:
 
   A. mixed multi-tensor job tables (ct_batched through ops.batched / ops.BatchedPlan): several kernel signatures, flat and 2-D
      scale addressing, partial and single-chunk tiles, unit-size fallbacks, misaligned views and empty tensors in ONE call;
-  B. the same tables under explicitly tuned TMA rings, the static deal, the direct pipeline and a CUDA-graph replay;
+  B. what those tables cover of the ring shapes and tile schedules the library launches with, and a CUDA-graph replay;
   C. the host-resident pipelines: ct_host_run (one large CPU tensor, chunked), ct_host_run_many (a CPU-resident model through
      ops.host_batched, chunks of many tensors sharing staging slots) and ModelCompressor on a CPU-resident model.
 
@@ -199,6 +199,7 @@ T_QPACK = [
     S("A1", (100, 200), BF, "block", (64, 64)),                      # blocks that do not: 25 chunks a row, sig.group = 1
     S("B2z", (64, 512), FP16, "channel", bits=8, zp=torch.int8),
     S("C1", (48, 256), FP32, "group", 128),
+    S("C1", (896, 8192), FP32, "group", 128),                        # 896 tiles: wraps the 2-stage ring, static deal (section B)
     S("C8", (40, 96), FP32, "tensor", bits=8),
     S("generic", (8, 96), BF, "tensor", bits=3),                     # 3-bit codes
     S("generic", (5, 12), BF, "tensor"),                             # ragged: cols * bits % 32 != 0
@@ -210,8 +211,8 @@ T_QPACK = [
 ] + _many("A4", BF)
 L_QPACK = 11
 # under stream capture the job tables go up with one-warp upload kernels, one per 32 jobs of every group with >= 2 jobs:
-# A1 (3 jobs) 1, A4 (38 jobs) 2
-L_QPACK_CAPTURED = L_QPACK + 3
+# A1 (3 jobs) 1, A4 (38 jobs) 2, C1 (2 jobs) 1
+L_QPACK_CAPTURED = L_QPACK + 4
 
 # op 1, unpack + dequantize (no unit grouping; the 4-bit input of a job must be a multiple of 16 bytes for the bulk copy).
 # U4 = bf16/4/-, U4z = bf16/4/int8, V8z = fp16/8/int8, W4 = fp32/4/-.  4 signatures + 7 generic = 11 launches.
@@ -227,6 +228,7 @@ T_UNPACK = [
     S("U4z", (100, 200), BF, "block", (64, 64), zp=torch.int8),
     S("V8z", (64, 512), FP16, "channel", bits=8, zp=torch.int8),
     S("W4", (48, 256), FP32, "group", 128),
+    S("W4", (2048, 8192), FP32, "group", 128),                       # 2048 tiles: wraps the 4-stage ring, static deal (section B)
     S("generic", (8, 96), BF, "tensor", bits=3),
     S("generic", (5, 12), BF, "tensor"),
     S("generic", (16, 256), BF, "group", 128, odt=FP32),             # output dtype differs from the scale's
@@ -443,7 +445,8 @@ def _fp4_problem(entry, g, device=DEV):
 
 # op 9, unpack + dequantize FP4 (bulk copies need n % 32 == 0).  Signatures (output dtype, scale kind): Sb = bf16/bf16 scale,
 # F8b = bf16/stored fp8, E8b = bf16/stored E8M0, Sh = fp16/fp16 scale.  The kernel of a signature does not know whether a job has a
-# global scale: Sb jobs with and without one alternate over 1024 tiles, more than one per CTA.  4 signatures + 1 generic = 5 launches.
+# global scale: Sb jobs of 128 tiles with and without one alternate, and the static deal hands each CTA tiles of different jobs
+# (section B).  4 signatures + 1 generic = 5 launches.
 # (label, shape, scale kind, output dtype, group, global scale)
 T_FP4D = [("Sb", (512, 2048), "same", BF, 16, (i % 2 == 0)) for i in range(8)] + [
     ("F8b", (64, 256), "fp8", BF, 16, True),
@@ -611,33 +614,70 @@ def test_sparse24_int4_table_vs_oracle():
 # --------------------------------------------------------------------------------------------
 # B. ring shapes and schedules
 # --------------------------------------------------------------------------------------------
-# (pipe, stages, ctas_per_sm): 2-stage ring; the 12-stage maximum (cut back to what fits 200 KB); 4 CTAs an SM, which the shrink loop
-# has to cut for the 32 KB tiles of the 16-bit ops; the static deal over the TMA ring (pipe 2) for every launch size; the direct
-# pipeline with 8 CTAs an SM.  Several tiles a CTA everywhere, so every ring shape wraps around its stages (mbarrier phase flips).
-RINGS = [(1, 2, 1), (1, 12, 1), (1, 4, 4), (2, 4, 2), (0, 4, 8)]
+# The rings the library launches with (csrc/stream.cuh: ring_shape), as (tile chunks, stages, CTAs per SM) by op and element type;
+# the grid is min(SMs x CTAs, tiles).  A launch of fewer than DYNAMIC_MIN_TILES_PER_SM x 1024 chunks per SM keeps the static deal
+# (csrc/dispatch.cu): CTA c takes tiles c, c + grid, c + 2 grid, ...
+RINGS = {
+    (N.OP_QUANTIZE_PACK, BF): (2048, 3, 2),
+    (N.OP_QUANTIZE_PACK, FP16): (2048, 3, 2),
+    (N.OP_QUANTIZE_PACK, FP32): (1024, 2, 3),             # 4 x 3 asked for, cut to fit 200 KB of 32 KB tiles
+    (N.OP_UNPACK_DEQUANTIZE, BF): (2048, 3, 2),
+    (N.OP_UNPACK_DEQUANTIZE, FP16): (2048, 3, 2),
+    (N.OP_UNPACK_DEQUANTIZE, FP32): (1024, 4, 3),
+    (N.OP_UNPACK_DEQUANTIZE_FP4, BF): (1024, 4, 3),
+}
+DYNAMIC_MIN_TILES_PER_SM = 24
 
 
-@pytest.fixture(params=RINGS, ids=lambda r: "pipe%d-stages%d-ctas%d" % r)
-def ring(request):
-    N.set_tuning(*request.param)
-    try:
-        yield request.param
-    finally:
-        N.set_tuning(1, 4, 0)
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-@pytest.mark.parametrize("name", ["quantize_pack", "unpack_dequantize"])
-def test_mixed_table_under_ring_shape(ring, name):
-    _run_table(_table(name), f"{name} under {ring}")
+def _is_static(tiles, tile, sms):
+    return tiles * tile < DYNAMIC_MIN_TILES_PER_SM * 1024 * sms
 
 
-def test_mixed_table_fp4_decompress_under_static_deal():
-    """the static deal hands every CTA tiles of alternating jobs with and without a global scale"""
-    N.set_tuning(2, 4, 2)
-    try:
-        _run_fp4(N.OP_UNPACK_DEQUANTIZE_FP4, T_FP4D, _fp4d_problem, L_FP4D, "fp4 unpack_dequantize, static deal")
-    finally:
-        N.set_tuning(1, 4, 0)
+def test_tables_wrap_every_ring():
+    """A launch of more tiles than grid x stages gives some CTA more tiles than its ring has stages, whatever the schedule: that CTA
+    reuses a stage and waits on its barriers' flipped phase.  The op 0 and 1 tables (test_mixed_table_vs_oracle) have such a launch
+    on every ring those ops launch with, one of them under the static deal with several tiles a CTA."""
+    sms = _sms()
+    for name in ("quantize_pack", "unpack_dequantize"):
+        op, table, _ = TABLES[name]
+        tiles, dts = {}, {}
+        for s in table:
+            if s.label in ("generic", "empty"):
+                continue
+            tile = RINGS[(op, s.dt)][0]
+            tiles[s.label] = tiles.get(s.label, 0) + -(-(math.prod(s.shape) // 8) // tile)
+            dts.setdefault(s.label, set()).add(s.dt)
+        wrapped, static = set(), False
+        for label, n in tiles.items():
+            assert len(dts[label]) == 1, f"{name}: signature {label} mixes element types"
+            tile, stages, ctas = RINGS[(op, dts[label].pop())]
+            grid = min(sms * ctas, n)
+            if n > grid * stages:
+                wrapped.add((stages, ctas))
+                static = static or _is_static(n, tile, sms)
+        assert wrapped == {(st, ct) for (o, _), (_, st, ct) in RINGS.items() if o == op}, f"{name}: rings wrapped {wrapped}"
+        assert static, f"{name}: no statically dealt launch wraps its ring"
+
+
+def test_fp4_decompress_table_crosses_jobs_under_static_deal():
+    """In the Sb launch of T_FP4D, the static deal gives most CTAs consecutive tiles of one job with a global scale and one without,
+    so the FP4 decompress op must rebuild its per-tensor constants (Op::tile) when the job changes, not once per CTA
+    (test_mixed_fp4_unpack_dequantize_table_vs_oracle)."""
+    tile, _, ctas = RINGS[(N.OP_UNPACK_DEQUANTIZE_FP4, BF)]
+    sms = _sms()
+    owner = []                                                           # job of every tile of the launch
+    sb = [e for e in T_FP4D if e[0] == "Sb"]
+    for j, (_, (R, C), *_) in enumerate(sb):
+        owner += [j] * -(-(R * C // 8) // tile)
+    n = len(owner)
+    grid = min(sms * ctas, n)
+    assert _is_static(n, tile, sms) and n > grid, (n, grid)
+    crossing = sum(any(sb[owner[t]][5] != sb[owner[t + grid]][5] for t in range(c, n - grid, grid)) for c in range(grid))
+    assert crossing > grid // 2, f"{crossing} of {grid} CTAs cross between jobs with and without a global scale"
 
 
 def test_mixed_table_cuda_graph_replay():

@@ -32,13 +32,6 @@ def cuda(t):
     return None if t is None else t.to(DEV)
 
 
-@pytest.fixture(params=["tma", "direct"])
-def pipe(request):
-    N.set_tuning(1 if request.param == "tma" else 0, 4, 0)
-    yield request.param
-    N.set_tuning(1, 4, 0)
-
-
 # --------------------------------------------------------------------------------------------
 # 0. the arithmetic proof the fast path rests on
 # --------------------------------------------------------------------------------------------
@@ -92,7 +85,7 @@ def test_quant_golden_gpu(c):
     same(fq.cpu(), c["fq"], "fake_quantize: ")
 
 
-def test_sweep_golden_gpu(pipe):
+def test_sweep_golden_gpu():
     """every bf16 / fp16 bit pattern x 4 scales, int4 / int8+zp / fp8 / fake-quant; every int8 and fp8 code"""
     sw = load("sweep")
     pat = torch.arange(65536, dtype=torch.int32).to(torch.uint16)
@@ -140,7 +133,7 @@ def test_bitmask_golden_gpu():
 
 
 # --------------------------------------------------------------------------------------------
-# 2. seeded inputs vs the oracle, fast (streaming) path, both pipelines
+# 2. seeded inputs vs the oracle, fast (streaming) path
 # --------------------------------------------------------------------------------------------
 def _weights(shape, dtype, seed):
     g = torch.Generator().manual_seed(seed)
@@ -164,7 +157,7 @@ def _group_qparams(w, bits, group, sym, dtype):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
 @pytest.mark.parametrize("bits,sym", [(4, True), (4, False), (8, True), (8, False)])
-def test_quantize_pack_vs_oracle(pipe, dtype, bits, sym):
+def test_quantize_pack_vs_oracle(dtype, bits, sym):
     w = _weights((1024, 4096), dtype, 1000 + bits)
     scale, zp = _group_qparams(w, bits, 128, sym, dtype)
     a = ns(strategy="group", group_size=128, num_bits=bits, symmetric=sym)
@@ -186,7 +179,7 @@ def test_quantize_pack_vs_oracle(pipe, dtype, bits, sym):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
 @pytest.mark.parametrize("strategy", ["tensor", "channel", "group"])
-def test_fp8_quantize_dequantize_vs_oracle(pipe, dtype, strategy):
+def test_fp8_quantize_dequantize_vs_oracle(dtype, strategy):
     w = _weights((1024, 4096), dtype, 77)
     if strategy == "tensor":
         scale = (w.float().abs().max() / 448).to(dtype).reshape(1)
@@ -211,7 +204,7 @@ def test_fp8_quantize_dequantize_vs_oracle(pipe, dtype, strategy):
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
 @pytest.mark.parametrize("sym", [True, False])
-def test_int8_channel_quantize_vs_oracle(pipe, dtype, sym):
+def test_int8_channel_quantize_vs_oracle(dtype, sym):
     w = _weights((512, 4096), dtype, 5)
     wf = w.float()
     mn, mx = wf.amin(-1, keepdim=True).clamp(max=0), wf.amax(-1, keepdim=True).clamp(min=0)
@@ -248,7 +241,7 @@ def test_extreme_scales_take_the_ieee_division_path():
 
 @pytest.mark.parametrize("bits", [1, 2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("shape", [(64, 4096), (33, 100), (7, 1), (128, 33)])
-def test_pack_unpack_vs_oracle(pipe, bits, shape):
+def test_pack_unpack_vs_oracle(bits, shape):
     g = torch.Generator().manual_seed(bits * 7 + shape[1])
     q = torch.randint(-(1 << (bits - 1)), 1 << (bits - 1), shape, dtype=torch.int8, generator=g)
     for pd in (1, 0):

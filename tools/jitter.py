@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """
 Per-launch timing distribution of the multi-tensor ops on one H100 (one CUDA-event pair per launch):
-tells a systematic slowdown from sporadic stalls.  Prints one JSON line per (op, pipe).
+tells a systematic slowdown from sporadic stalls.  Prints one JSON line per op.
 """
 import argparse
 import json
@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-import sweep  # noqa: E402
+import headline_problems  # noqa: E402
 from compressed_tensors_b200 import _native as N  # noqa: E402
 from compressed_tensors_b200 import ops  # noqa: E402
 
@@ -23,13 +23,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, default=8)
     ap.add_argument("--launches", type=int, default=40)
-    ap.add_argument("--pipes", default="1,2")
-    ap.add_argument("--tune", default="", help="comma list of stages:ctas_per_sm to compare on the streaming ops (per-launch medians), e.g. 4:3,6:2,8:2")
-    ap.add_argument("--ops", default="", help="with --tune: comma list of streaming ops to time (default: the seven headline ops)")
     a = ap.parse_args()
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
-    P, OPS, n = sweep.build_problems(a.layers)
+    P, OPS, n = headline_problems.build_problems(a.layers)
     codes = [torch.randint(-8, 8, (14336, 4096), dtype=torch.int8, device=dev) for _ in range(16)]
     pk = [torch.empty(c.shape[0], c.shape[1] // 8, dtype=torch.int32, device=dev) for c in codes]
     descs = []
@@ -69,56 +66,35 @@ def main():
     uv, um, uo = ops.bitmask_compress(un)
     extra_fns["bitmask_compress_50pct"] = (lambda: ops.bitmask_compress(un), nsp * (2 + 1 + 0.125))
     extra_fns["bitmask_decompress_50pct"] = (lambda: ops.bitmask_decompress(uv, um, uo, un.shape), nsp * (1 + 0.125 + 2))
-    if a.tune:
-        for cfg in a.tune.split(","):
-            st, ct = (int(v) for v in cfg.split(":"))
-            N.set_tuning(1, st, ct)
-            rec = {"stages": st, "ctas_per_sm": ct}
-            for name in (a.ops.split(",") if a.ops else ("quantpack", "unpackdeq", "fp8_q", "fp8_dq", "fake_w4", "nvfp4_qp", "nvfp4_ud")):
-                op, probs, nbytes = jobs[name]
-                for _ in range(3):
-                    ops.batched(op, probs, 0)
-                torch.cuda.synchronize()
-                ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.launches)]
-                for e0, e1 in ev:
-                    e0.record()
-                    ops.batched(op, probs, 0)
-                    e1.record()
-                torch.cuda.synchronize()
-                ms = sorted(e0.elapsed_time(e1) for e0, e1 in ev)
-                rec[name] = round(nbytes / ms[len(ms) // 2] / 1e6, 1)
-            print(json.dumps(rec), flush=True)
-        return
-    for pipe in [int(p) for p in a.pipes.split(",")]:
-        N.set_tuning(pipe, 4, 3)
-        for name, (op, probs, nbytes) in jobs.items():
-            for _ in range(3):
-                ops.batched(op, probs, 0)
-            torch.cuda.synchronize()
-            ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.launches)]
-            for e0, e1 in ev:
-                e0.record()
-                ops.batched(op, probs, 0)
-                e1.record()
-            torch.cuda.synchronize()
-            ms = [e0.elapsed_time(e1) for e0, e1 in ev]
-            s = sorted(ms)
-            print(json.dumps({"op": name, "pipe": {1: "tma-dynamic", 2: "tma-static"}[pipe], "GBps_best": round(nbytes / s[0] / 1e6, 1),
-                              "GBps_median": round(nbytes / s[len(s) // 2] / 1e6, 1), "GBps_worst": round(nbytes / s[-1] / 1e6, 1),
-                              "ms": [round(v, 3) for v in ms]}), flush=True)
-        for name, (fn, nbytes) in extra_fns.items():
-            for _ in range(3):
-                fn()
-            torch.cuda.synchronize()
-            ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.launches)]
-            for e0, e1 in ev:
-                e0.record()
-                fn()
-                e1.record()
-            torch.cuda.synchronize()
-            s = sorted(e0.elapsed_time(e1) for e0, e1 in ev)
-            print(json.dumps({"op": name, "pipe": "plain grid launch (includes the output allocation)", "GBps_best": round(nbytes / s[0] / 1e6, 1),
-                              "GBps_median": round(nbytes / s[len(s) // 2] / 1e6, 1)}), flush=True)
+    for name, (op, probs, nbytes) in jobs.items():
+        for _ in range(3):
+            ops.batched(op, probs, 0)
+        torch.cuda.synchronize()
+        ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.launches)]
+        for e0, e1 in ev:
+            e0.record()
+            ops.batched(op, probs, 0)
+            e1.record()
+        torch.cuda.synchronize()
+        ms = [e0.elapsed_time(e1) for e0, e1 in ev]
+        s = sorted(ms)
+        print(json.dumps({"op": name, "GBps_best": round(nbytes / s[0] / 1e6, 1),
+                          "GBps_median": round(nbytes / s[len(s) // 2] / 1e6, 1), "GBps_worst": round(nbytes / s[-1] / 1e6, 1),
+                          "ms": [round(v, 3) for v in ms]}), flush=True)
+    # plain grid launches: their times include the output allocation
+    for name, (fn, nbytes) in extra_fns.items():
+        for _ in range(3):
+            fn()
+        torch.cuda.synchronize()
+        ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(a.launches)]
+        for e0, e1 in ev:
+            e0.record()
+            fn()
+            e1.record()
+        torch.cuda.synchronize()
+        s = sorted(e0.elapsed_time(e1) for e0, e1 in ev)
+        print(json.dumps({"op": name, "GBps_best": round(nbytes / s[0] / 1e6, 1),
+                          "GBps_median": round(nbytes / s[len(s) // 2] / 1e6, 1)}), flush=True)
 
 
 if __name__ == "__main__":

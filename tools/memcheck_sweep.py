@@ -133,10 +133,7 @@ def batched_family(dt):
         out = torch.empty(rows, cols // 8, dtype=torch.int32, device=DEV)
         p = ops._resolve(x, s, None, a, None)
         probs.append((ops._desc(p, dt, dt, None, dt, torch.int8, None, N.Q_INT, 4), x, s, None, out))
-    for pipe in (1, 2, 0):
-        N.set_tuning(pipe, 4, 3)
-        ops.batched(N.OP_QUANTIZE_PACK, probs, 0)
-    N.set_tuning(1, 4, 3)
+    ops.batched(N.OP_QUANTIZE_PACK, probs, 0)
     # round 2: the fused 2:4 + int4 ops as multi-tensor launches (bitmask in desc.aux)
     c24, d24, keep = [], [], []
     for d, x, s, _, _ in probs:

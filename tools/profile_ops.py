@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 from compressed_tensors_b200 import _native as N  # noqa: E402
 from compressed_tensors_b200 import ops  # noqa: E402
-from tools.sweep import build_problems  # noqa: E402
+from tools.headline_problems import build_problems  # noqa: E402
 
 
 def main():
