@@ -172,6 +172,11 @@ __device__ __forceinline__ void bulk_g2s_a(uint32_t smem_dst, const void* gsrc, 
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
         ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar), "l"(policy) : "memory");
 }
+// the same copy at the default L2 priority
+__device__ __forceinline__ void bulk_g2s_a(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar) : "memory");
+}
 // shared -> global bulk store (bulk async-group completion)
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");

@@ -121,6 +121,7 @@ struct QuantPackOp {
     static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
+    static constexpr bool INPUT_EVICT_FIRST = false;   // reads 2-8x what it writes: see InputEvictFirst
     static constexpr int IN_BYTES = 8 * ElemBytes<P>::v;
     static constexpr int GROUP = G;
     static constexpr int OUT_WORDS = BITS / 4;   // per chunk
