@@ -120,7 +120,6 @@ _PROTOS = {
     "ct_bitmask_compress_onepass": (_int, [_vp, _int, _vp, _vp, _vp, _vp, _i64, _i64, _int, _vp]),
     "ct_semi_structured_from_dense": (_int, [_vp, _int, _vp, _vp, _i64, _i64, _int, _vp]),
     "ct_semi_structured_to_dense": (_int, [_vp, _int, _vp, _vp, _i64, _i64, _int, _vp]),
-    "ct_host_run": (_int, [_int, _descp, _vp, _vp, _vp, _vp, _int]),
     "ct_host_run_many": (_int, [_int, _int, _descp, _vp, _vp, _vp, _vp, _int]),
     "ct_selftest_division": (_int, [_int, ctypes.POINTER(ctypes.c_uint64), _int]),
     "ct_selftest_fp4_division": (_int, [_int, _int, _int, ctypes.POINTER(ctypes.c_uint64), _int]),

@@ -11,7 +11,7 @@ and error behaviour as the reference's per-tensor functions
 resolution and output allocation.  All arithmetic happens in libct_b200.so on a H100.
 
 Device policy: CUDA tensors run on their device and the current stream.  CPU tensors are staged
-through the current CUDA device (large 2-D tensors via the pipelined ct_host_run) and the result
+through the current CUDA device (large 2-D tensors via the pipelined ct_host_run_many) and the result
 is returned on the CPU, as the reference would.  With no CUDA device the call raises; there is
 no eager / CPU fallback.  Meta tensors only get their output shape and dtype computed.
 """
@@ -319,11 +319,9 @@ def _run(fn_name: str, op: int, d: N.QuantDesc, p: _Problem, src: torch.Tensor, 
     ):
         # pipelined H2D / kernel / D2H on host buffers
         srcc = src.contiguous()
-        sc = p.scale.contiguous()
         zp = p.zp.contiguous() if p.zp is not None else None
         out = torch.empty(out_shape, dtype=out_dtype, pin_memory=srcc.is_pinned())
-        rc = lib.ct_host_run(op, ctypes.byref(d), N.ptr(srcc), N.ptr(sc), N.ptr(zp), N.ptr(out), idx)
-        N.check(rc, fn_name)
+        host_batched(op, [(d, srcc, p.scale.contiguous(), zp, out)], idx)
         return out
     s_dev = _to_dev(src, idx)
     sc = _to_dev(p.scale, idx)
@@ -996,6 +994,14 @@ def _validate_problem(op: int, i: int, prob, on_cuda: Optional[int]) -> None:
             bad(f"{what} lives on {t.device}, host_batched expects CPU tensors")
 
 
+def _tables(problems):
+    """the ctypes tables of a job list: descriptors, then the in / scale / zp / out pointers (0 for an absent tensor)"""
+    n = max(len(problems), 1)
+    vp = ctypes.c_void_p * n
+    ptrs = [vp(*[(p[k].data_ptr() if p[k] is not None else 0) for p in problems]) for k in (1, 2, 3, 4)]
+    return ((N.QuantDesc * n)(*[p[0] for p in problems]), *ptrs)
+
+
 class BatchedPlan:
     """A validated multi-tensor launch that can be enqueued any number of times (`run()`): the descriptors are checked against their
     tensors once, the pointer tables are built once, and `run()` is a single ct_batched call on the current stream.  The plan keeps
@@ -1010,13 +1016,7 @@ class BatchedPlan:
         for i, p in enumerate(problems):
             _validate_problem(self.op, i, p, self.idx)
         self._keep = list(problems)
-        n = self.n
-        vp = ctypes.c_void_p * max(n, 1)
-        self._descs = (N.QuantDesc * max(n, 1))(*[p[0] for p in problems])
-        self._ins = vp(*[p[1].data_ptr() for p in problems])
-        self._scs = vp(*[(p[2].data_ptr() if p[2] is not None else 0) for p in problems])
-        self._zps = vp(*[(p[3].data_ptr() if p[3] is not None else 0) for p in problems])
-        self._outs = vp(*[p[4].data_ptr() for p in problems])
+        self._descs, self._ins, self._scs, self._zps, self._outs = _tables(problems)
 
     def run(self) -> None:
         if self.n == 0:
@@ -1046,12 +1046,7 @@ def host_batched(op: int, problems: Sequence[Tuple[N.QuantDesc, torch.Tensor, to
     for i, p in enumerate(problems):
         _validate_problem(int(op), i, p, None)
     idx = device_index if device_index is not None else N.require_device(None)
-    descs = (N.QuantDesc * n)(*[p[0] for p in problems])
-    vp = ctypes.c_void_p * n
-    ins = vp(*[p[1].data_ptr() for p in problems])
-    scs = vp(*[p[2].data_ptr() for p in problems])
-    zps = vp(*[(p[3].data_ptr() if p[3] is not None else 0) for p in problems])
-    outs = vp(*[p[4].data_ptr() for p in problems])
+    descs, ins, scs, zps, outs = _tables(problems)
     rc = N.lib().ct_host_run_many(int(op), n, descs, ctypes.cast(ins, ctypes.c_void_p), ctypes.cast(scs, ctypes.c_void_p),
                                   ctypes.cast(zps, ctypes.c_void_p), ctypes.cast(outs, ctypes.c_void_p), idx)
     N.check(rc, "ct_host_run_many")

@@ -288,17 +288,13 @@ int ct_semi_structured_from_dense(const void* dense, int dtype, void* sparse, vo
 int ct_semi_structured_to_dense(const void* sparse, int dtype, const void* meta, void* dense, int64_t m, int64_t k,
                                 int device, void* stream);
 
-/* ---- host-buffer entry points (what a CPU-resident caller of the reference API hits) ----
- * Same semantics as ct_batched with n == 1, but every pointer is a HOST pointer (pinned memory
- * gives full PCIe rate; pageable works).  Rows are streamed through the device in chunks with
- * H2D copy / kernel / D2H copy overlapped on three streams.  Blocking. */
-int ct_host_run(int op, const ct_quant_desc* d, const void* in, const void* scale, const void* zp, void* out,
-                int device);
-
-/* The same op over n host-resident tensors (a CPU-resident model: the body of ModelCompressor.compress_model /
- * decompress_model for state dicts that live in host memory), pipelined ACROSS tensors: all row chunks form one
- * queue through 4 staging slots, so the PCIe copy engines do not drain between tensors.  Blocking. */
-/* (for the FP4 ops d->global_scale is a HOST pointer here, like every other pointer of these two entry points) */
+/* ---- host-buffer entry point (what a CPU-resident caller of the reference API hits) ----
+ * Same semantics as ct_batched, but every pointer is a HOST pointer (pinned memory gives full PCIe rate; pageable works),
+ * d->global_scale of the FP4 ops included.  n == 1 for one large CPU tensor; a CPU-resident model (the body of
+ * ModelCompressor.compress_model / decompress_model for state dicts that live in host memory) passes all its tensors.
+ * Rows are streamed through the device in chunks, and the chunks of all tensors form one queue through 4 staging slots
+ * (H2D copy / kernel / D2H copy on a stream each), so the PCIe copy engines do not drain between tensors.  Blocking, on
+ * error too: no copy from or into the caller's buffers is left in flight.  Serialises per device on its staging buffers. */
 int ct_host_run_many(int op, int n, const ct_quant_desc* descs, const void* const* in, const void* const* scale,
                      const void* const* zp, void* const* out, int device);
 

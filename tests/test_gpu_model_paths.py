@@ -4,8 +4,9 @@ The paths a whole model takes, element by element against the CPU oracle:
   A. mixed multi-tensor job tables (ct_batched through ops.batched / ops.BatchedPlan): several kernel signatures, flat and 2-D
      scale addressing, partial and single-chunk tiles, unit-size fallbacks, misaligned views and empty tensors in ONE call;
   B. what those tables cover of the ring shapes and tile schedules the library launches with, and a CUDA-graph replay;
-  C. the host-resident pipelines: ct_host_run (one large CPU tensor, chunked), ct_host_run_many (a CPU-resident model through
-     ops.host_batched, chunks of many tensors sharing staging slots) and ModelCompressor on a CPU-resident model.
+  C. the host-resident pipeline ct_host_run_many: one large CPU tensor through the per-tensor ops (chunked), a CPU-resident model
+     through ops.host_batched (chunks of many tensors sharing staging slots, an error part-way) and ModelCompressor on a
+     CPU-resident model.
 
 Every table entry names the kernel it is meant to take (a signature label, "generic" or "empty").  The number of launches a
 call makes is written next to each table, derived by hand from the planner's rules in csrc/dispatch.cu (plan_one / plan_fp4 /
@@ -717,8 +718,9 @@ def _need_memory(gib):
         pytest.skip(f"needs {gib} GB of free device memory")
 
 
-# ct_host_run: 32 MiB chunks.  bf16 [5000, 7168] with 128-row blocks -> chunks of 2432, 2432 and 136 rows, the last one crossing a
-# partial block; int8 / 8-bit packed [9650, 7168] -> 4681 rows a chunk (4736 with 128-row blocks), ragged last chunk.
+# one CPU tensor through the per-tensor ops: 32 MiB chunks.  bf16 [5000, 7168] with 128-row blocks -> chunks of 2432, 2432 and
+# 136 rows, the last one crossing a partial block; int8 / 8-bit packed [9650, 7168] -> 4681 rows a chunk (4736 with 128-row
+# blocks), ragged last chunk.
 HOST_CASES = {
     "quantize_pack": [("block", True), ("group", False), ("tensor", True)],
     "unpack_dequantize": [("channel", True), ("group1", False), ("group", True)],     # the strategy is inferred from the scale shape
@@ -802,18 +804,31 @@ HOST_MANY_0_4 = {
 }
 
 
-@pytest.mark.parametrize("slots", [2, 3, 8])
-def test_host_batched_vs_oracle(slots, monkeypatch):
+HOST_SLOTS = 4   # staging slots of the pipeline (csrc/host_pipeline.cu: NSLOT)
+
+
+def _host_chunks(d, src, chunk=1 << 20):
+    """row chunks the pipeline cuts one table entry into, by the rule above"""
+    if d.rows * d.cols == 0:
+        return 0
+    rpc = max(chunk // (src.numel() * src.element_size() // d.rows), 1)
+    if d.rdiv != N.INF and d.rdiv > 1:
+        rpc = -(-rpc // d.rdiv) * d.rdiv
+    return -(-d.rows // rpc)
+
+
+def test_host_batched_vs_oracle(monkeypatch):
     monkeypatch.setenv("CT_B200_HOST_CHUNK_MB", "1")
-    monkeypatch.setenv("CT_B200_HOST_SLOTS", str(slots))
-    g = torch.Generator().manual_seed(slots)
+    g = torch.Generator().manual_seed(HOST_SLOTS)
     for op, table in HOST_MANY_0_4.items():
         probs, wants, outs = [], [], []
         for s in table:
             pr, w, o = _problem(op, s, g, device="cpu")
             probs.append(pr); wants.append(w); outs.append(o)
+        chunks = sum(_host_chunks(pr[0], pr[1]) for pr in probs)
+        assert chunks > 2 * HOST_SLOTS, f"op {op}: {chunks} chunks do not reuse every one of the {HOST_SLOTS} staging slots"
         ops.host_batched(op, probs)
-        _check(outs, wants, table, f"host_batched op {op}, {slots} slots")
+        _check(outs, wants, table, f"host_batched op {op}")
     # FP4: every NVFP4 tensor carries its own global scale as a HOST pointer
     for op, table, builder in ((N.OP_QUANTIZE_PACK_FP4, [("nv", "h", (1024, 2048), BF, BF, 16, None, 1.0), ("nv", "h", (700, 1536), BF, FP32, 16, F8, 20.0),
                                                          ("mx", "h", (512, 1024), BF, BF, 32, torch.uint8, 1.0), ("nv", "h", (0, 64), BF, BF, 16, None, 1.0),
@@ -827,7 +842,27 @@ def test_host_batched_vs_oracle(slots, monkeypatch):
             probs.append(pr); wants.append(w); outs.append(o); keep.append(k)
         ops.host_batched(op, probs)
         for i, (o, w) in enumerate(zip(outs, wants)):
-            same(o, w, f"host_batched op {op}, {slots} slots, entry {i} {table[i][:3]}")
+            same(o, w, f"host_batched op {op}, entry {i} {table[i][:3]}")
+
+
+def test_host_batched_error_part_way_leaves_no_copy_in_flight(monkeypatch):
+    """a table whose second entry fails the library's dtype check after the first entry's chunks are queued (pinned buffers, so
+    the copies are truly asynchronous): host_batched raises only once those copies have landed, and the pipeline works after it"""
+    monkeypatch.setenv("CT_B200_HOST_CHUNK_MB", "1")
+    g = torch.Generator().manual_seed(12)
+    s = S("h", (2000, 2048), BF, "group", 128, bits=8)
+    pr, want, _ = _problem(N.OP_QUANTIZE, s, g, device="cpu")
+    good = tuple(t.pin_memory() if isinstance(t, torch.Tensor) else t for t in pr)
+    assert _host_chunks(good[0], good[1]) >= 2 * HOST_SLOTS
+    (d, _, sc, _, out), _, _ = _problem(N.OP_QUANTIZE, S("h", (64, 256), BF, "group", 128, bits=8), g, device="cpu")
+    d.x_dtype = N.DT[torch.int8]                                  # right size for the int8 input below, but not a float to quantize
+    bad = (d, torch.zeros((64, 256), dtype=torch.int8).pin_memory(), sc.pin_memory(), None, out.pin_memory())
+    with pytest.raises(ValueError, match="dtype must be float"):
+        ops.host_batched(N.OP_QUANTIZE, [good, bad])
+    same(good[4], want, "first entry, right after the error")
+    good[4].view(torch.uint8).fill_(0xA5)
+    ops.host_batched(N.OP_QUANTIZE, [good])
+    same(good[4], want, "the same entry, called again")
 
 
 @pytest.mark.parametrize("pinned", [True, False], ids=["pinned", "pageable"])

@@ -407,7 +407,7 @@ def test_batched_launch_equals_per_tensor():
 
 
 def test_host_buffers_pipeline_equals_device_path():
-    """CPU tensors go through ct_host_run (chunked H2D / kernel / D2H) and must give identical bytes"""
+    """CPU tensors go through ct_host_run_many (chunked H2D / kernel / D2H) and must give identical bytes"""
     w = _weights((12288, 4096), torch.bfloat16, 31)   # 96 MiB -> 3 chunks
     scale = (w.float().unflatten(-1, (-1, 128)).abs().amax(-1) / 7.5).bfloat16()
     a = ns(strategy="group", group_size=128, num_bits=4)
