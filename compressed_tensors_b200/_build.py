@@ -29,6 +29,7 @@ SOURCES = [
     "fast_pack.cu",
     "fast_quant.cu",
     "fast_fake.cu",
+    "fake_heads.cu",
     "dispatch.cu",
     "selftest.cu",
     "host_pipeline.cu",

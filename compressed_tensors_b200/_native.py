@@ -70,6 +70,25 @@ class QuantDesc(ctypes.Structure):
     ]
 
 
+class HeadJob(ctypes.Structure):
+    """mirror of `struct ct_head_job` (include/ct_b200.h)"""
+
+    _fields_ = [
+        ("x", ctypes.c_void_p),
+        ("out", ctypes.c_void_p),
+        ("scale", ctypes.c_void_p),
+        ("zp", ctypes.c_void_p),
+        ("shape", ctypes.c_int64 * 4),
+        ("stride", ctypes.c_int64 * 4),
+        ("per_head", ctypes.c_int32),
+        ("x_dtype", ctypes.c_int32),
+        ("scale_dtype", ctypes.c_int32),
+        ("zp_dtype", ctypes.c_int32),
+        ("qtype", ctypes.c_int32),
+        ("num_bits", ctypes.c_int32),
+    ]
+
+
 class NativeLibraryError(RuntimeError):
     pass
 
@@ -90,6 +109,7 @@ _PROTOS = {
     "ct_quantize": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_dequantize": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_fake_quantize": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
+    "ct_fake_quantize_heads": (_int, [_int, ctypes.POINTER(HeadJob), _int, _vp]),
     "ct_quantize_pack_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_unpack_dequantize_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_observe_quantize_pack_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),

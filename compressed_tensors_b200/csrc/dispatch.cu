@@ -69,7 +69,7 @@ static uint32_t bits_of(int dt, float v) {
     return 0;
 }
 
-static Common make_common(int p_dt, int qtype, int bits) {
+Common make_common(int p_dt, int qtype, int bits) {
     Common cm;
     if (qtype == CT_Q_INT) {
         const float r = (float)(1 << bits);

@@ -66,6 +66,7 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
                 const void* const* zp, const int32_t* const* g_idx, void* const* out, int device, cudaStream_t stream);
 
 int check_device(int device);
+Common make_common(int p_dt, int qtype, int bits);   // clamp bounds of a (qtype, bits) in the compute dtype p_dt (dispatch.cu)
 
 // ---- CPU twins (cpu_twin.cu): host code behind device = CT_DEVICE_CPU, same per-element source as the generic kernels ----
 int cpu_run_bits(bool pack, const void* in, void* out, int64_t rows, int64_t cols, int bits, int packed_dim);

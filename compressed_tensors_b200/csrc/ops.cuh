@@ -39,16 +39,17 @@ __device__ __forceinline__ uint32_t scale_index(const Job& J, uint32_t gc) {
 }
 
 template <class P, int ZP>
-__device__ __forceinline__ RawQP fetch_qp(const Job& J, uint32_t gc) {
+__device__ __forceinline__ RawQP load_qp(const void* scale, const void* zp, uint32_t si) {
     RawQP r;
-    const uint32_t si = scale_index(J, gc);
-    if constexpr (P::DT == CT_F32) r.s = __float_as_uint(__ldg(reinterpret_cast<const float*>(J.scale) + si));
-    else r.s = __ldg(reinterpret_cast<const unsigned short*>(J.scale) + si);
+    if constexpr (P::DT == CT_F32) r.s = __float_as_uint(__ldg(reinterpret_cast<const float*>(scale) + si));
+    else r.s = __ldg(reinterpret_cast<const unsigned short*>(scale) + si);
     r.z = 0;
-    if constexpr (ZP == 1) r.z = __ldg(reinterpret_cast<const int8_t*>(J.zp) + si);
-    if constexpr (ZP == 2) r.z = __ldg(reinterpret_cast<const uint8_t*>(J.zp) + si);
+    if constexpr (ZP == 1) r.z = __ldg(reinterpret_cast<const int8_t*>(zp) + si);
+    if constexpr (ZP == 2) r.z = __ldg(reinterpret_cast<const uint8_t*>(zp) + si);
     return r;
 }
+template <class P, int ZP>
+__device__ __forceinline__ RawQP fetch_qp(const Job& J, uint32_t gc) { return load_qp<P, ZP>(J.scale, J.zp, scale_index(J, gc)); }
 template <class P> __device__ __forceinline__ float scale_f32(const RawQP& r) {
     if constexpr (P::DT == CT_BF16) return __uint_as_float(r.s << 16);
     else if constexpr (P::DT == CT_F16) return __half2float(__ushort_as_half((unsigned short)r.s));
@@ -408,9 +409,8 @@ struct FakeQuantOp {
     __device__ static __forceinline__ Raw prefetch(const Job& J, uint32_t gc) { return fetch_qp<P, ZP>(J, gc); }
 
     template <bool SLOW>
-    __device__ static __forceinline__ void body(const Job& J, const Common& cm, const ScaleCtx& sc, uint32_t s2, uint32_t zp2, uint32_t gc,
-                                                const uint32_t (&w)[IN_BYTES / 4]) {
-        uint32_t o[IN_BYTES / 4];
+    __device__ static __forceinline__ void body(const Common& cm, const ScaleCtx& sc, uint32_t s2, uint32_t zp2,
+                                                const uint32_t (&w)[IN_BYTES / 4], uint32_t (&o)[IN_BYTES / 4]) {
         if constexpr (P::DT == CT_F32) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -428,13 +428,18 @@ struct FakeQuantOp {
                 o[k] = dq_tail2<P, ZP>(t, zp2, s2);
             }
         }
-        store_out8<P>(J.out, gc, o);
     }
-    __device__ static __forceinline__ void run(const Job& J, const Common& cm, const Raw& r, uint32_t gc, const uint32_t (&wg)[1][IN_BYTES / 4], int) {
+    // one chunk w -> o with the raw scale / zero point r; the streaming run() below and the strided kernel of fake_heads.cu share it
+    __device__ static __forceinline__ void apply(const Common& cm, const Raw& r, const uint32_t (&w)[IN_BYTES / 4], uint32_t (&o)[IN_BYTES / 4]) {
         const ScaleCtx sc = make_scale_ctx(scale_f32<P>(r));
         const uint32_t s2 = scale_t2<P>(r), zp2 = zp_t2<P, ZP>(r);
-        if (sc.slow && P::DT != CT_F32) body<true>(J, cm, sc, s2, zp2, gc, wg[0]);
-        else body<false>(J, cm, sc, s2, zp2, gc, wg[0]);
+        if (sc.slow && P::DT != CT_F32) body<true>(cm, sc, s2, zp2, w, o);
+        else body<false>(cm, sc, s2, zp2, w, o);
+    }
+    __device__ static __forceinline__ void run(const Job& J, const Common& cm, const Raw& r, uint32_t gc, const uint32_t (&wg)[1][IN_BYTES / 4], int) {
+        uint32_t o[IN_BYTES / 4];
+        apply(cm, r, wg[0], o);
+        store_out8<P>(J.out, gc, o);
     }
 };
 

@@ -33,6 +33,7 @@ __all__ = [
     "quantize",
     "dequantize",
     "fake_quantize",
+    "fake_quantize_heads",
     "quantize_pack",
     "unpack_dequantize",
     "pack_bitmasks",
@@ -455,6 +456,70 @@ def fake_quantize(x, scale, zero_point, args, g_idx=None, global_scale=None) -> 
     x2 = x.reshape(p.rows, p.cols)
     out = _run("ct_fake_quantize", N.OP_FAKE_QUANTIZE, d, p, x2, (p.rows, p.cols), out_dtype)
     return out.reshape(x.shape)
+
+
+def _head_job(x: torch.Tensor, scale: torch.Tensor, zp: Optional[torch.Tensor], args, out: torch.Tensor):
+    """(the ct_head_job of one [B, H, S, D] tensor, the flattened scale / zero point it points into), or None when the strided kernel
+    cannot take the tensor (the library checks the layout).  Scale shapes: one element (TENSOR), or [H, 1, 1] / [1, H, 1, 1] with the
+    ATTN_HEAD strategy -- the shapes `fake_quantize` broadcasts one scale per head; any other shape takes `fake_quantize`."""
+    if x.ndim != 4 or not x.is_cuda or x.dtype not in _FLOAT_DTYPES or scale.dtype != x.dtype or out.stride() != x.stride():
+        return None
+    if scale.device != x.device or (zp is not None and (zp.device != x.device or zp.dtype not in (torch.int8, torch.float8_e4m3fn))):
+        return None
+    if zp is not None and zp.shape != scale.shape:
+        return None
+    heads = x.shape[1]
+    if scale.numel() == 1:
+        per_head = 0
+    elif _strategy_name(args) == "attn_head" and tuple(scale.shape) in ((heads, 1, 1), (1, heads, 1, 1)):
+        per_head = 1
+    else:
+        return None
+    qtype, bits = _qparams(args)
+    if qtype == N.Q_FP4:
+        return None
+    flat_scale = scale.reshape(-1).contiguous()
+    flat_zp = zp.reshape(-1).contiguous() if zp is not None else None
+    j = N.HeadJob()
+    j.x, j.out, j.scale = x.data_ptr(), out.data_ptr(), flat_scale.data_ptr()
+    j.zp = flat_zp.data_ptr() if flat_zp is not None else None
+    j.shape[:] = list(x.shape)
+    j.stride[:] = list(x.stride())
+    j.per_head = per_head
+    j.x_dtype = j.scale_dtype = N.DT[x.dtype]
+    j.zp_dtype = N.DT[zp.dtype] if zp is not None else N.DT_NONE
+    j.qtype, j.num_bits = qtype, bits
+    return j, (flat_scale, flat_zp)
+
+
+@torch.no_grad()
+def fake_quantize_heads(tensors: Sequence[torch.Tensor], scales: Sequence[torch.Tensor], zero_points: Sequence[Optional[torch.Tensor]],
+                        args) -> list:
+    """
+    fake_quantize of one or two attention states (key and value, or query) of shape [B, H, S, D] in one launch, where they lie:
+    transformers hands them over as transposed, non-contiguous views, and this reads and writes them with their own strides
+    (ct_fake_quantize_heads) instead of copying each one to a contiguous buffer first.  Scales are per tensor ([1], TENSOR) or
+    per head ([H, 1, 1], ATTN_HEAD); the outputs are `torch.empty_like` their inputs and equal `fake_quantize` bit for bit.
+    Inputs the strided kernel does not take (CPU tensors, other strategies, scale shapes or dtypes, D % 8 != 0, unaligned or
+    non-dense rows) run through `fake_quantize` one by one, with the scales and zero points exactly as given.
+    """
+    tensors, scales, zero_points = list(tensors), list(scales), list(zero_points)
+    if not 1 <= len(tensors) <= 2 or len(scales) != len(tensors) or len(zero_points) != len(tensors):
+        raise ValueError("fake_quantize_heads takes one or two tensors, each with its scale and zero point (or None)")
+    if any(x.device.type == "meta" for x in tensors) or all(x.numel() == 0 for x in tensors):
+        return [fake_quantize(x, s, z, args) for x, s, z in zip(tensors, scales, zero_points)]
+    strategy = _strategy_name(args)
+    if strategy in ("tensor", "attn_head") and len({x.device for x in tensors}) == 1 and not getattr(_mode, "cpu", False):
+        outs = [torch.empty_like(x) for x in tensors]
+        jobs = [_head_job(x, s, z, args, o) for x, s, z, o in zip(tensors, scales, zero_points, outs)]
+        if all(j is not None for j in jobs):
+            idx = tensors[0].device.index
+            table = (N.HeadJob * len(jobs))(*(j for j, _ in jobs))   # `jobs` keeps the flattened qparams alive until the launch
+            rc = N.lib().ct_fake_quantize_heads(len(jobs), table, idx, N.stream_ptr(idx))
+            if rc != N.CT_E_UNSUPPORTED:
+                N.check(rc, "ct_fake_quantize_heads")
+                return outs
+    return [fake_quantize(x, s, z, args) for x, s, z in zip(tensors, scales, zero_points)]
 
 
 # --------------------------------------------------------------------------------------------

@@ -1,7 +1,7 @@
 """
 apply_quantization_config: walk a model, match module names / class names against the config's
 targets and ignore list, attach schemes and qparams (mirror of quantization/lifecycle/apply.py:100-169
-restricted to Linear / Embedding targets -- attention / kv-cache hooks are outside this engine's path).
+for Linear / Embedding targets, attention modules and the KV cache -- the last two through the hooks of `modeling/`).
 
 Target syntax (utils/match.py of the reference): a target matches a module when it equals the
 module name, equals the class name, or is "re:<regex>" matching either.
@@ -15,47 +15,67 @@ from copy import deepcopy
 import torch
 from torch.nn import Module
 
-from ...utils.match import is_match, match_named_modules, match_targets
+from ...utils.match import is_match, is_narrow_match, match_named_modules, match_targets
+from ..quant_args import QuantizationArgs
 from ..quant_config import QuantizationConfig, QuantizationStatus
-from .initialize import initialize_module_for_quantization
+from ..quant_scheme import QuantizationScheme
+from ..utils.helpers import KV_CACHE_TARGETS
+from .initialize import initialize_module_for_quantization, is_cached_attention_module
 
 __all__ = ["apply_quantization_config", "is_match", "match_named_modules", "load_pretrained_quantization_parameters"]
 
 _LOGGER = logging.getLogger(__name__)
 
 
-def _looks_like_attention(module: Module) -> bool:
-    """the reference's `_is_attention_module` test (quantization/lifecycle/initialize.py:123-130): class name contains "attention"
-    and the module owns k_proj / v_proj / qkv_proj"""
-    return "attention" in module.__class__.__name__.lower() and any(hasattr(module, n) for n in ("k_proj", "v_proj", "qkv_proj"))
-
-
 def apply_quantization_config(model: Module, config: QuantizationConfig | None, run_compressed: bool = False, show_progress: bool = False):
-    """quantization/lifecycle/apply.py:100-169.  A module that matches several targets takes the scheme of the most specific one
+    """quantization/lifecycle/apply.py:100-192.  A module that matches several targets takes the scheme of the most specific one
     (`match_targets`: exact name, then regex on the name, then class name -- apply.py:149-151, :258-265), not the first in config
-    order.  KV-cache schemes and attention-module targets are outside this engine's path (SURVEY 2, OUT OF SCOPE): they raise /
-    warn instead of being dropped silently."""
+    order.  A `kv_cache_scheme` is applied to every cached attention module first; a config group that narrowly targets a cached
+    attention module hooks its query, key and value states (modeling/).  Unlike the reference, a `kv_cache_scheme` that no module
+    of the model can take raises instead of being dropped."""
     config = deepcopy(config)
     if config is None:
         return dict()
     force_zero_point = config.quantization_status < QuantizationStatus.COMPRESSED
     if getattr(config, "kv_cache_scheme", None) is not None:
-        raise NotImplementedError(
-            "compressed_tensors_b200 does not implement KV-cache quantization (the reference's _apply_kv_cache_scheme / "
-            "initialize_hooked_kv_cache, apply.py:172-192): a checkpoint with `kv_cache_scheme` cannot be loaded by this engine")
+        _apply_kv_cache_scheme(model, config.kv_cache_scheme, config.quantization_status)
     target_to_scheme = OrderedDict()
     for scheme in config.config_groups.values():
         for target in scheme.targets:
             target_to_scheme[target] = scheme
     for name, module in match_named_modules(model, target_to_scheme, config.ignore, warn_on_fail=True):
         scheme = target_to_scheme[match_targets(name, module, target_to_scheme)[0]]
-        if isinstance(module, (torch.nn.Linear, torch.nn.Embedding)):
+        if is_cached_attention_module(module) and is_narrow_match(model, scheme.targets, name):
+            from ...modeling import initialize_hooked_attention
+
+            module.quantization_scheme = scheme
+            initialize_hooked_attention(model, module)
+            initialize_module_for_quantization(module, force_zero_point=force_zero_point)
+            module.quantization_status = config.quantization_status
+        elif isinstance(module, (torch.nn.Linear, torch.nn.Embedding)):
             module.quantization_scheme = scheme
             initialize_module_for_quantization(module, force_zero_point=force_zero_point)
             module.quantization_status = config.quantization_status
-        elif _looks_like_attention(module):
-            _LOGGER.warning(f"{name}: attention-module quantization targets are not supported by compressed_tensors_b200; "
-                            "no q/k/v scales are attached (the reference would run initialize_hooked_attention here)")
+
+
+def _apply_kv_cache_scheme(model: Module, kv_cache_scheme: QuantizationArgs, status: QuantizationStatus) -> None:
+    """k / v qparams and a QuantizedKVCache on every cached attention module (apply.py:172-192).  Runs before the config groups, so
+    that an attention target initialised afterwards keeps its own q / k / v qparams."""
+    if not kv_cache_scheme.symmetric:
+        _LOGGER.warning("vLLM does not support asymmetric kv cache quantization")
+    from ...modeling import initialize_hooked_kv_cache
+
+    scheme = QuantizationScheme(targets=list(KV_CACHE_TARGETS), input_activations=kv_cache_scheme)
+    modules = [m for m in model.modules() if is_cached_attention_module(m)]
+    if not modules:
+        raise NotImplementedError(
+            "KV-cache quantization: the config has a `kv_cache_scheme`, but no attention module of this model could take it (an "
+            "attention module whose forward takes `past_key_values`); refusing to drop the scheme silently")
+    for module in modules:
+        module.quantization_scheme = scheme
+        initialize_hooked_kv_cache(model, module)
+        initialize_module_for_quantization(module, force_zero_point=False)
+        module.quantization_status = status
 
 
 def load_pretrained_quantization_parameters(model: Module, model_name_or_path: str | None = None, load_weight_qparams: bool = False) -> None:

@@ -6,18 +6,24 @@ for Linear / Embedding modules): `weight_scale`, `weight_zero_point`, `weight_g_
 """
 from __future__ import annotations
 
+import inspect
+import logging
 import math
 
 import torch
 from torch.nn import Module, Parameter
 
+from ...utils.helpers import deprecated, get_head_dim, get_num_attn_heads, get_num_kv_heads
 from ..quant_args import ActivationOrdering, DynamicType, QuantizationArgs, QuantizationStrategy
 from ..quant_config import QuantizationStatus
 from ..quant_scheme import QuantizationScheme
 from ..utils.helpers import strategy_cdiv
 from .forward import set_forward_quantized
 
-__all__ = ["initialize_module_for_quantization", "initialize_qparams", "QPARAM_SUFFIXES"]
+__all__ = ["initialize_module_for_quantization", "initialize_qparams", "initialize_attn_qparams", "is_cached_attention_module",
+           "is_attention_module", "QPARAM_SUFFIXES"]
+
+_LOGGER = logging.getLogger(__name__)
 
 QPARAM_SUFFIXES = ("_scale", "_zero_point", "_global_scale", "_g_idx")
 _BASE_NAMES = ("weight", "input", "output", "q", "k", "v")
@@ -36,24 +42,86 @@ def initialize_module_for_quantization(module: Module, scheme: QuantizationSchem
     if scheme is None:
         return
     _clear_qparams(module)
-    if not isinstance(module, (torch.nn.Linear, torch.nn.Embedding)):
+    if is_cached_attention_module(module):
+        initialize_attn_qparams(module, scheme, force_zero_point)
+    elif isinstance(module, (torch.nn.Linear, torch.nn.Embedding)):
+        weight = module.weight
+        if scheme.input_activations is not None:
+            initialize_qparams(module, "input", scheme.input_activations, weight.shape[-1:], weight.dtype, force_zero_point)
+        if scheme.weights is not None:
+            initialize_qparams(module, "weight", scheme.weights, weight.shape, weight.dtype, force_zero_point)
+        if scheme.output_activations is not None:
+            initialize_qparams(module, "output", scheme.output_activations, weight.shape[:-1], weight.dtype, force_zero_point)
+        set_forward_quantized(module)
+    else:
         raise ValueError(f"Quantization of module type {type(module)} is not supported")
-    weight = module.weight
-    if scheme.input_activations is not None:
-        initialize_qparams(module, "input", scheme.input_activations, weight.shape[-1:], weight.dtype, force_zero_point)
-    if scheme.weights is not None:
-        initialize_qparams(module, "weight", scheme.weights, weight.shape, weight.dtype, force_zero_point)
-    if scheme.output_activations is not None:
-        initialize_qparams(module, "output", scheme.output_activations, weight.shape[:-1], weight.dtype, force_zero_point)
-    set_forward_quantized(module)
     module.quantization_scheme = scheme
     module.quantization_status = QuantizationStatus.INITIALIZED
+
+
+def _is_attention_module(module: Module) -> bool:
+    """class name contains "attention" and the module owns one of the K / V projections (initialize.py:123-130 of the reference)"""
+    return "attention" in module.__class__.__name__.lower() and any(
+        hasattr(module, n) for n in ("k_proj", "v_proj", "qkv_proj", "kv_b_proj"))
+
+
+@deprecated("is_cached_attention_module")
+def is_attention_module(module: Module) -> bool:
+    return _is_attention_module(module)
+
+
+def is_cached_attention_module(module: Module) -> bool:
+    """an attention module whose forward takes a KV cache (`past_key_values`, or `past_key_value` before transformers#39956): the
+    modules that K / V quantization hooks can attach to"""
+    if not _is_attention_module(module):
+        return False
+    try:
+        parameters = inspect.signature(module.forward).parameters
+    except (TypeError, ValueError):
+        _LOGGER.warning("Unable to inspect an attention module's forward signature; skipping KV cache quantization for uninspectable modules")
+        return False
+    return "past_key_value" in parameters or "past_key_values" in parameters
+
+
+def _validate_attention_scheme(scheme: QuantizationScheme) -> None:
+    if scheme.weights is not None:
+        raise ValueError("Cannot apply weight quantization to attention. Instead, target the (q|k|v)_proj submodule layers of attention")
+    if scheme.input_activations is None:
+        raise ValueError("Cannot apply attention quantization without specifying input activations")
+    if scheme.output_activations is not None:
+        raise ValueError("Cannot apply output quantization to attention")
+
+
+def initialize_attn_qparams(module: Module, scheme: QuantizationScheme, force_zero_point: bool) -> None:
+    """`q_*` (when the module carries a QuantizedAttentionImpl) and `k_*` / `v_*` (QuantizedKVCache) qparams of an attention module,
+    shaped for states [batch, heads, seq, head_dim] of the decoder config the cache holds"""
+    from ...modeling import IMPL_ATTR, KV_CACHE_ATTR
+
+    impl = getattr(module, IMPL_ATTR, None)
+    kv_cache = getattr(module, KV_CACHE_ATTR, None)
+    if impl is None and kv_cache is None:
+        raise ValueError(f"Attention module has quantization scheme but no {IMPL_ATTR} or {KV_CACHE_ATTR} attributes. Please ensure that "
+                         "these attributes are initialized using `apply_quantization_config`.")
+    _validate_attention_scheme(scheme)
+    config = kv_cache.config
+    head_dim = get_head_dim(config)
+    dtype = next(module.parameters()).dtype
+    args = scheme.input_activations
+    if impl is not None:
+        initialize_qparams(module, "q", args, (get_num_attn_heads(config), None, head_dim), dtype, force_zero_point)
+    if kv_cache is not None:
+        kv_shape = (get_num_kv_heads(config), None, head_dim)
+        initialize_qparams(module, "k", args, kv_shape, dtype, force_zero_point)
+        initialize_qparams(module, "v", args, kv_shape, dtype, force_zero_point)
 
 
 def initialize_qparams(module: Module, base_name: str, quantization_args: QuantizationArgs, observed_shape, observed_dtype: torch.dtype,
                        force_zero_point: bool = True):
     strategy, dynamic = quantization_args.strategy, quantization_args.dynamic
-    device = module.weight.device if getattr(module, "weight", None) is not None else None
+    if getattr(module, "weight", None) is not None:
+        device = module.weight.device
+    else:   # attention modules: the device of their projections
+        device = next(module.parameters(), torch.empty(0)).device
     if dynamic is True:
         return
     if strategy == QuantizationStrategy.TENSOR_GROUP:

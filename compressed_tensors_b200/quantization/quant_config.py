@@ -117,23 +117,32 @@ class QuantizationConfig(BaseModel):
 
     @staticmethod
     def from_pretrained(model: Module, format: str | list | None = None) -> "QuantizationConfig | None":
-        """rebuild the config from the `quantization_scheme` attached to each module (quant_config.py:186-289)"""
+        """rebuild the config from the `quantization_scheme` attached to each module (quant_config.py:186-289).  A quantized cached
+        attention module gives the `kv_cache_scheme`; it also forms a config group when its query is hooked (an attention target)."""
+        from ..modeling import IMPL_ATTR
+        from .lifecycle.initialize import is_cached_attention_module
         from .utils.helpers import is_module_quantized
 
         schemes: list[QuantizationScheme] = []
         status = None
+        kv_cache_scheme: QuantizationArgs | None = None
         quantized_types: set[str] = set()
         unquantized: dict[str, list[str]] = defaultdict(list)
         for name, sub in model.named_modules():
             kind = _vllm_module_type(type(sub).__name__)
-            if is_module_quantized(sub):
+            quantized = is_module_quantized(sub)
+            cached_attention = quantized and is_cached_attention_module(sub)
+            if quantized and (not cached_attention or hasattr(sub, IMPL_ATTR)):
                 status = getattr(sub, "quantization_status", status)
                 quantized_types.add(kind)
                 if sub.quantization_scheme not in schemes:
                     schemes.append(sub.quantization_scheme)
             else:
                 unquantized[kind].append(name)
-        if not schemes:
+            if cached_attention:
+                status = getattr(sub, "quantization_status", status)
+                kv_cache_scheme = sub.quantization_scheme.input_activations
+        if not schemes and kv_cache_scheme is None:
             return None
         ignore = [n for kind, names in unquantized.items() if kind in quantized_types for n in names]
         groups = {f"group_{i}": s for i, s in enumerate(schemes)}
@@ -143,7 +152,7 @@ class QuantizationConfig(BaseModel):
         elif isinstance(format, list):
             format = CompressionFormat.mixed_precision.value if len(format) > 1 else format[0]
         ignore = _map_to_checkpoint_names(model, ignore)
-        return QuantizationConfig(config_groups=groups, quantization_status=status, kv_cache_scheme=None,
+        return QuantizationConfig(config_groups=groups, quantization_status=status, kv_cache_scheme=kv_cache_scheme,
                                   global_compression_ratio=None, format=format, ignore=ignore)
 
     def requires_calibration_data(self) -> bool:

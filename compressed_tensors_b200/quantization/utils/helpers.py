@@ -30,7 +30,11 @@ __all__ = [
     "module_type",
     "get_torch_bit_depth",
     "can_quantize",
+    "KV_CACHE_TARGETS",
 ]
+
+# nominal targets of the scheme a `kv_cache_scheme` becomes on attention modules (apply_quantization_config never matches them)
+KV_CACHE_TARGETS = ["re:.*(self_attn|attention)$"]
 
 
 def calculate_range(quantization_args: QuantizationArgs, device) -> tuple[Tensor, Tensor]:

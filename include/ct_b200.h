@@ -132,6 +132,30 @@ int ct_dequantize(const ct_quant_desc* d, const void* q, const void* scale, cons
 int ct_fake_quantize(const ct_quant_desc* d, const void* x, const void* scale, const void* zp, const int32_t* g_idx,
                      void* out, int device, void* stream);
 
+/* ---- attention K / V / Q fake quantization in place of their strided layout ----------------
+ * replaces the forward_quantize calls of modeling/kvcache.py (QuantizedKVCache.forward: key and value states) and
+ * modeling/attention.py (QuantizedAttentionImpl.forward: query states).  transformers hands those tensors over as the
+ * transposed views [B, H, S, D] of [B, S, H, D] projections, which are not contiguous; one launch fake-quantizes every job
+ * where it lies, with ct_fake_quantize's per-element arithmetic (bit-identical), and writes `out` with the same strides.
+ *   scale / zp: per_head = 0 -> one element (TENSOR); per_head = 1 -> H elements (ATTN_HEAD, scale [H, 1, 1]); zp may be NULL
+ * Supported: x_dtype == scale_dtype in {F32, F16, BF16}; CT_Q_INT with 1..8 bits or CT_Q_FLOAT (fp8 e4m3, 8 bits); zp_dtype
+ * CT_I8 (or CT_F8E4M3 for CT_Q_FLOAT); stride[3] == 1, D % 8 == 0, x / out 16-byte aligned and the other strides a multiple
+ * of 16 bytes; fewer than 2^31 / 8 elements per job; all jobs of a call share dtypes, qtype, bits and the zero-point kind.
+ * Anything else returns CT_E_UNSUPPORTED (the caller then runs ct_fake_quantize on contiguous copies).  n is 1 or 2.
+ * Enqueue-only, no host synchronisation. */
+typedef struct ct_head_job {
+    const void* x;
+    void* out;
+    const void* scale;
+    const void* zp;
+    int64_t shape[4];       /* B, H, S, D */
+    int64_t stride[4];      /* element strides of x and out */
+    int32_t per_head;
+    int32_t x_dtype, scale_dtype, zp_dtype;   /* zp_dtype CT_NONE without a zero point */
+    int32_t qtype, num_bits;
+} ct_head_job;
+int ct_fake_quantize_heads(int n, const ct_head_job* jobs, int device, void* stream);
+
 /* ---- fused compressor bodies ------------------------------------------------
  * quantize(dtype=int8) -> pack_to_int32 in one pass (pack_quantized/base.py:96-104) and
  * unpack_from_int32 -> dequantize (pack_quantized/base.py:159-166); the int8
