@@ -30,6 +30,7 @@ SOURCES = [
     "fast_quant.cu",
     "fast_fake.cu",
     "fake_heads.cu",
+    "hadamard.cu",
     "dispatch.cu",
     "selftest.cu",
     "host_pipeline.cu",

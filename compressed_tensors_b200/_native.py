@@ -44,6 +44,7 @@ DT = {
 
 Q_INT, Q_FLOAT, Q_FP4 = 0, 1, 2
 DT_E8M0 = 8  # uint8 MX scale exponent as stored (CT_E8M0)
+DT_F64 = 9   # compute precision of ct_hadamard_transform (CT_F64)
 
 
 class QuantDesc(ctypes.Structure):
@@ -89,6 +90,23 @@ class HeadJob(ctypes.Structure):
     ]
 
 
+class HadamardJob(ctypes.Structure):
+    """mirror of `struct ct_hadamard_job` (include/ct_b200.h)"""
+
+    _fields_ = [
+        ("x", ctypes.c_void_p),
+        ("out", ctypes.c_void_p),
+        ("shape", ctypes.c_int64 * 4),
+        ("stride", ctypes.c_int64 * 4),
+        ("sign", ctypes.c_void_p),
+        ("perm", ctypes.c_void_p),
+        ("dtype", ctypes.c_int32),
+        ("precision", ctypes.c_int32),
+        ("log2_n", ctypes.c_int32),
+        ("inverse", ctypes.c_int32),
+    ]
+
+
 class NativeLibraryError(RuntimeError):
     pass
 
@@ -110,6 +128,7 @@ _PROTOS = {
     "ct_dequantize": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_fake_quantize": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_fake_quantize_heads": (_int, [_int, ctypes.POINTER(HeadJob), _int, _vp]),
+    "ct_hadamard_transform": (_int, [ctypes.POINTER(HadamardJob), _int, _vp]),
     "ct_quantize_pack_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_unpack_dequantize_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_observe_quantize_pack_int32": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),

@@ -8,9 +8,11 @@
 // The arithmetic is the SAME SOURCE as the generic CUDA kernels: quant_at / dequant_at / pack_group / unpack_group of generic.cuh and
 // quant_core.cuh are __host__ __device__, so the per-op rounding, the clamp-before-round order, the wrapping-sum bit packing and the
 // scale addressing cannot drift between the two.  OpenMP over rows.  Nothing under oracle/ is linked or included.
+#include <cmath>
 #include <cstring>
 
 #include "generic.cuh"
+#include "hadamard.cuh"
 
 namespace ctb {
 
@@ -174,6 +176,64 @@ int cpu_run_one(int op, const ct_quant_desc& d, const void* in, const void* scal
     }
     set_error("op %d has no CPU twin (device = -1 covers pack / unpack, quantize / dequantize / fake_quantize and the two fused compressor bodies)", op);
     return CT_E_UNSUPPORTED;
+}
+
+// ct_hadamard_transform on the host: the butterfly order of hadamard.cu (stage h = 1, 2, ..., n/2), the same conversions (hadamard.cuh)
+template <class C, int DT>
+static void cpu_hadamard_rows(const ct_hadamard_job& j) {
+    using E = Elem<DT>;
+    using T = typename E::T;
+    const int64_t n = (int64_t)1 << j.log2_n;
+    const int64_t per_row = j.shape[3] >> j.log2_n;
+    const int64_t rows = j.shape[0] * j.shape[1] * j.shape[2] * per_row;
+    const C scale = (C)std::sqrt((double)n);
+    const T* x = reinterpret_cast<const T*>(j.x);
+    T* out = reinterpret_cast<T*>(j.out);
+#pragma omp parallel
+    {
+        C* z = new C[n];
+#pragma omp for schedule(static)
+        for (int64_t r = 0; r < rows; ++r) {
+            const int64_t bhs = r / per_row, k = r % per_row;
+            const int64_t s = bhs % j.shape[2], bh = bhs / j.shape[2];
+            const int64_t h = bh % j.shape[1], b = bh / j.shape[1];
+            const int64_t off = b * j.stride[0] + h * j.stride[1] + s * j.stride[2] + k * n;
+            for (int64_t i = 0; i < n; ++i) {
+                const int64_t q = j.perm ? j.perm[i] : i;
+                C v = E::template load<C>(x[off + i]);
+                if (j.sign && !j.inverse && j.sign[q] < 0) v = -v;
+                z[q] = v;
+            }
+            for (int64_t hh = 1; hh < n; hh <<= 1)
+                for (int64_t i = 0; i < n; ++i)
+                    if (!(i & hh)) {
+                        const C a = z[i], c = z[i + hh];
+                        z[i] = a + c;
+                        z[i + hh] = a - c;
+                    }
+            for (int64_t i = 0; i < n; ++i) {
+                const int64_t q = j.perm ? j.perm[i] : i;
+                C v = z[q];
+                if (j.sign && j.inverse && j.sign[q] < 0) v = -v;
+                out[off + i] = E::store(v / scale);
+            }
+        }
+        delete[] z;
+    }
+}
+
+template <class C>
+static void cpu_hadamard_dt(const ct_hadamard_job& j) {
+    switch (j.dtype) {
+    case CT_BF16: cpu_hadamard_rows<C, CT_BF16>(j); break;
+    case CT_F16: cpu_hadamard_rows<C, CT_F16>(j); break;
+    default: cpu_hadamard_rows<C, CT_F32>(j); break;
+    }
+}
+
+void cpu_hadamard(const ct_hadamard_job& j) {
+    if (j.precision == CT_F64) cpu_hadamard_dt<double>(j);
+    else cpu_hadamard_dt<float>(j);
 }
 
 }  // namespace ctb

@@ -71,6 +71,7 @@ Common make_common(int p_dt, int qtype, int bits);   // clamp bounds of a (qtype
 // ---- CPU twins (cpu_twin.cu): host code behind device = CT_DEVICE_CPU, same per-element source as the generic kernels ----
 int cpu_run_bits(bool pack, const void* in, void* out, int64_t rows, int64_t cols, int bits, int packed_dim);
 int cpu_run_one(int op, const ct_quant_desc& d, const void* in, const void* scale, const void* zp, const int32_t* g_idx, void* out);
+void cpu_hadamard(const ct_hadamard_job& j);   // ct_hadamard_transform on host pointers (job already validated)
 
 // ---- unstructured bitmask in one pass (bitmask_onepass.cu): decoupled look-back over per-tile counts ----------------
 bool bitmask_lookback_ok(int dtype, int64_t rows, int64_t cols, const void* dense, const void* mask, const void* values);

@@ -10,7 +10,7 @@ import contextlib
 
 import torch
 
-__all__ = ["update_offload_parameter", "disable_onloading", "get_execution_device", "is_distributed"]
+__all__ = ["update_offload_parameter", "disable_onloading", "disable_offloading", "get_execution_device", "is_distributed"]
 
 
 def update_offload_parameter(module: torch.nn.Module, name: str, data: torch.Tensor):
@@ -24,6 +24,12 @@ def update_offload_parameter(module: torch.nn.Module, name: str, data: torch.Ten
 @contextlib.contextmanager
 def disable_onloading():
     """nothing is ever offloaded here, so there is nothing to disable"""
+    yield
+
+
+@contextlib.contextmanager
+def disable_offloading():
+    """nothing is ever offloaded here, so there is nothing to keep onloaded"""
     yield
 
 

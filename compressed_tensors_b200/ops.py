@@ -34,6 +34,7 @@ __all__ = [
     "dequantize",
     "fake_quantize",
     "fake_quantize_heads",
+    "hadamard_transform",
     "quantize_pack",
     "unpack_dequantize",
     "pack_bitmasks",
@@ -71,7 +72,7 @@ _HOST_PIPELINE_MIN_BYTES = 8 << 20
 # --------------------------------------------------------------------------------------------
 # device staging
 # --------------------------------------------------------------------------------------------
-_CPU = -1              # CT_DEVICE_CPU: the explicit host twins of the seven per-tensor hot-path entry points (csrc/cpu_twin.cu)
+_CPU = -1              # CT_DEVICE_CPU: the explicit host twins of the seven per-tensor hot-path entry points and of ct_hadamard_transform (csrc/cpu_twin.cu)
 _mode = threading.local()
 
 
@@ -520,6 +521,90 @@ def fake_quantize_heads(tensors: Sequence[torch.Tensor], scales: Sequence[torch.
                 N.check(rc, "ct_fake_quantize_heads")
                 return outs
     return [fake_quantize(x, s, z, args) for x, s, z in zip(tensors, scales, zero_points)]
+
+
+# --------------------------------------------------------------------------------------------
+# Walsh-Hadamard transforms (transform/factory/hadamard.py, HadamardTransform.forward)
+# --------------------------------------------------------------------------------------------
+HADAMARD_MAX_ORDER = 1 << 15
+
+
+def _hadamard_job(x: torch.Tensor, out: torch.Tensor, log2_n: int, sign, perm, inverse: bool, precision) -> N.HadamardJob:
+    j = N.HadamardJob()
+    j.x, j.out = x.data_ptr(), out.data_ptr()
+    j.shape[:] = list(x.shape)
+    j.stride[:] = list(x.stride())
+    j.sign = sign.data_ptr() if sign is not None else None
+    j.perm = perm.data_ptr() if perm is not None else None
+    j.dtype = N.DT[x.dtype]
+    j.precision = N.DT_F64 if precision == torch.float64 else N.DT[torch.float32]
+    j.log2_n, j.inverse = log2_n, int(bool(inverse))
+    return j
+
+
+def _check_permutation(perm: torch.Tensor, n: int) -> None:
+    """perm must be a permutation of 0 .. n-1 (the kernel scatters and gathers through it).  The values are checked once per version of
+    the tensor: callers that pass the same device copy every call (HadamardTransform) pay for one check."""
+    if perm.dtype not in (torch.int64, torch.int32) or perm.ndim != 1 or perm.numel() != n:
+        raise ValueError(f"perm must be a 1-D integer permutation of {n} indices, got shape {tuple(perm.shape)} and dtype {perm.dtype}")
+    if perm.device.type == "meta":
+        return
+    key = (perm._version, perm.data_ptr())
+    if getattr(perm, "_ct_checked_permutation", None) == key:
+        return
+    if not torch.equal(torch.sort(perm).values, torch.arange(n, device=perm.device, dtype=perm.dtype)):
+        raise ValueError(f"perm is not a permutation of 0 .. {n - 1}")
+    perm._ct_checked_permutation = key
+
+
+@torch.no_grad()
+def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = None, perm: Optional[torch.Tensor] = None,
+                       inverse: bool = False, precision: torch.dtype = torch.float32) -> torch.Tensor:
+    """
+    `(x.to(precision) @ M / sqrt(n)).to(x.dtype)` along the last dimension, block-diagonal over its n-element blocks, for the structured
+    matrices of the `hadamard` / `random-hadamard` factories: M = H (Sylvester), with rows and columns permuted by `perm` (a permutation
+    of 0 .. n-1) and / or rows signed by `sign` (n values, negative -> -1, else +1: diag(sign) . H); `inverse` applies M^T.  A `sign`
+    or `perm` of another length, or a `perm` that is not a permutation, raises ValueError.  An O(n log n) butterfly
+    (ct_hadamard_transform) instead of the dense product; precision fp32 or fp64.  The output has x's strides when x is dense (the
+    transposed [B, H, S, D] attention states included), so no contiguous copy is made in or out.
+    """
+    n = int(n)
+    if n <= 0 or n & (n - 1):
+        raise ValueError("Cannot construct deterministic hadamard of size != 2^n")
+    if n > HADAMARD_MAX_ORDER or n < 2:
+        raise NotImplementedError(f"hadamard_transform covers orders 2 .. {HADAMARD_MAX_ORDER}, got {n}")
+    _check_float(x, "input")
+    if precision not in (torch.float32, torch.float64):
+        raise NotImplementedError(f"hadamard_transform computes in float32 or float64, got {precision}")
+    if x.ndim == 0 or x.shape[-1] % n:
+        raise ValueError(f"{n} must divide the last dimension of a tensor of shape {tuple(x.shape)}")
+    if sign is not None and (sign.numel() != n or sign.dtype not in (torch.int8, torch.float32, torch.float64, torch.float16, torch.bfloat16)):
+        raise ValueError(f"sign must hold {n} signs, got {sign.numel()} of dtype {sign.dtype}")
+    if perm is not None:
+        _check_permutation(perm, n)
+    if x.device.type == "meta" or x.numel() == 0:
+        return torch.empty_like(x)
+    idx = _dev_index(x)
+    src = x
+    if idx == _CPU or not x.is_cuda:
+        src = _to_dev(x, idx)
+    if src.ndim > 4:
+        src = src.reshape(-1, *src.shape[-3:])
+    v = src.view((1,) * (4 - src.ndim) + tuple(src.shape)) if src.ndim < 4 else src
+    out = torch.empty_like(v)
+    if out.stride() != v.stride():          # not dense (a slice): the output cannot keep the input's strides
+        v = v.contiguous()
+        out = torch.empty_like(v)
+    sg = _to_dev(torch.where(sign < 0, -1, 1).to(torch.int8) if sign is not None and sign.dtype != torch.int8 else sign, idx)
+    pm = _to_dev(perm.to(torch.int64) if perm is not None else None, idx)
+    log2_n = n.bit_length() - 1
+    rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision)), idx, _stream(idx))
+    if rc == N.CT_E_UNSUPPORTED and not v.is_contiguous():
+        v = v.contiguous()
+        out = torch.empty_like(v)
+        rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision)), idx, _stream(idx))
+    N.check(rc, "hadamard_transform")
+    return _back(out.view(x.shape), x)
 
 
 # --------------------------------------------------------------------------------------------
@@ -1283,7 +1368,7 @@ def sparse24_unpack_dequantize(packed: torch.Tensor, bitmask: torch.Tensor, scal
 
 
 # --------------------------------------------------------------------------------------------
-# ImplBackend wiring (reference utils/impl_backend.py:23-134): the seven per-tensor hot-path ops are entrypoints.
+# ImplBackend wiring (reference utils/impl_backend.py:23-134): the seven per-tensor hot-path ops and hadamard_transform are entrypoints.
 #   backend "<op>_sm100": the CUDA kernels; req = a CUDA device is usable (CPU tensors are then staged through it, as before)
 #   eager body "<op>_eager": the library's own host code (device = -1 twins, csrc/cpu_twin.cu) -- what a GPU-less host and
 #                            CT_ENFORCE_EAGER=1 get.  Results are bit-identical (same per-element source as the generic kernels).
@@ -1295,7 +1380,8 @@ def _cuda_usable(*args, **kwargs) -> bool:
 def _wire_impl_backend():
     from .utils.impl_backend import ImplBackend
 
-    for name in ("pack_to_int32", "unpack_from_int32", "quantize", "dequantize", "fake_quantize", "quantize_pack", "unpack_dequantize"):
+    for name in ("pack_to_int32", "unpack_from_int32", "quantize", "dequantize", "fake_quantize", "quantize_pack", "unpack_dequantize",
+                 "hadamard_transform"):
         fn = globals()[name]
 
         def cuda_fn(*a, _fn=fn, **k):

@@ -1,8 +1,9 @@
 """
-Schema of the reference's transform configs (mirror of transform/transform_args.py, transform_scheme.py, transform_config.py).
-Only the schema: `ModelCompressor.update_config` carries a model's transform_config through to config.json
-(model_compressor.py:230-241).  Building and applying the transforms themselves (Hadamard / random rotations, fused weights) is a
-separate subsystem of the reference and out of scope here (DESIGN.md section 7).
+Transforms of the reference's transform/ package: the config schema (mirror of transform_args.py, transform_scheme.py,
+transform_config.py; `ModelCompressor.update_config` carries a model's transform_config through to config.json), the three factories
+(`hadamard`, `random-hadamard`, `random-matrix`, factory/) and `apply_transform_config` (apply.py).  Weight locations are fused into
+the weights, online locations run as hooks; the two Hadamard factories run on the Walsh-Hadamard kernel (`ops.hadamard_transform`)
+whenever their matrices have the structured form (DESIGN.md section 5).
 """
 from __future__ import annotations
 
@@ -13,7 +14,11 @@ from pydantic import BaseModel, ConfigDict, Field, field_validator
 
 from ..quantization.quant_args import TorchDtype
 
-__all__ = ["TransformLocation", "TransformArgs", "TransformScheme", "TransformConfig"]
+__all__ = [
+    "TransformLocation", "TransformArgs", "TransformScheme", "TransformConfig",
+    "TransformFactory", "TransformBase", "HadamardFactory", "HadamardTransform", "RandomHadamardFactory", "RandomMatrixFactory",
+    "RandomMatrixTransform", "apply_transform_config",
+]
 
 
 class TransformLocation(str, Enum):
@@ -70,3 +75,11 @@ class TransformConfig(BaseModel):
                 i += 1
                 name = f"{key}_{i}"
             self.config_groups[name] = scheme
+
+
+# the factories and apply_transform_config import the schema above (same order as the reference's transform/__init__.py)
+from .factory.base import TransformBase, TransformFactory  # noqa: E402
+from .factory.hadamard import HadamardFactory, HadamardTransform  # noqa: E402
+from .factory.matrix_multiply import RandomMatrixFactory, RandomMatrixTransform  # noqa: E402
+from .factory.random_hadamard import RandomHadamardFactory  # noqa: E402
+from .apply import apply_transform_config  # noqa: E402

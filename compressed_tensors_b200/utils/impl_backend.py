@@ -7,7 +7,7 @@ Op-level backend hook, same surface and semantics as the reference's ImplBackend
                                                  arguments, and always when CT_ENFORCE_EAGER is set (impl_backend.py:14-20, :98-123)
     ImplBackend.call(fn_name, ...)               call one registered function by its __name__, bypassing the checks (tests)
 
-In this engine the sm_90a kernels are the backend (registered by ops.py for the seven per-tensor hot-path ops with
+In this engine the sm_90a kernels are the backend (registered by ops.py for the seven per-tensor hot-path ops and hadamard_transform with
 req = "a CUDA device is usable") and the eager body is the library's OWN host code, the `device = -1` twins of the C ABI
 (csrc/cpu_twin.cu) -- not torch eager.  The reference reads CT_ENFORCE_EAGER once at import; here it is read at call time so that
 a test can flip it.

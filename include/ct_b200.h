@@ -21,7 +21,7 @@
  *     thread pool: entrypoints/convert/convert_checkpoint.py:110-134).
  *   - NO SILENT CPU FALLBACK: `device` >= 0 without a usable H100 fails with CT_E_NODEV, always.  The seven per-tensor
  *     entry points of the hot path (ct_pack_int32, ct_unpack_int32, ct_quantize, ct_dequantize, ct_fake_quantize,
- *     ct_quantize_pack_int32, ct_unpack_dequantize_int32, and ct_batched over them) have an EXPLICIT CPU twin: pass
+ *     ct_quantize_pack_int32, ct_unpack_dequantize_int32, and ct_batched over them) and ct_hadamard_transform have an EXPLICIT CPU twin: pass
  *     device = CT_DEVICE_CPU (-1) with HOST pointers and the call runs synchronously in host code of this library
  *     (csrc/cpu_twin.cu; same per-element source as the generic CUDA kernels), `stream` ignored.  That is the body the reference
  *     calls "eager" (utils/impl_backend.py:98-123): what a GPU-less host and CT_ENFORCE_EAGER=1 get.  Every other entry point
@@ -58,7 +58,8 @@ typedef enum ct_dtype_t {
     CT_I32 = 5,
     CT_U8 = 6,             /* also torch.bool */
     CT_I64 = 7,
-    CT_E8M0 = 8            /* uint8 biased power-of-two exponent: an MX scale as STORED (compressors/mx_utils.py:18-44) */
+    CT_E8M0 = 8,           /* uint8 biased power-of-two exponent: an MX scale as STORED (compressors/mx_utils.py:18-44) */
+    CT_F64 = 9             /* float64: only as the compute precision of ct_hadamard_transform */
 } ct_dtype_t;
 
 /* CT_Q_FLOAT = fp8 e4m3 (num_bits 8); CT_Q_FP4 = fp4 e2m1 (num_bits 4: values 0, .5, 1, 1.5, 2, 3, 4, 6 and negatives) */
@@ -155,6 +156,30 @@ typedef struct ct_head_job {
     int32_t qtype, num_bits;
 } ct_head_job;
 int ct_fake_quantize_heads(int n, const ct_head_job* jobs, int device, void* stream);
+
+/* ---- Walsh-Hadamard transforms of the transform factories ------------------------------------------------
+ * replaces HadamardTransform.forward (transform/factory/hadamard.py) -- apply_transform_weight / _multihead_matmul with a dense n x n
+ * matrix, then `/ sqrt(n)` and `.to(dtype)` -- for the structured matrices the `hadamard` and `random-hadamard` factories build:
+ *     y = x . M / sqrt(n) on every block of n consecutive elements of the last dimension (n = 2^log2_n, 1 <= log2_n <= 15, n | D)
+ *     M = H, H[perm][:, perm], diag(sign) . H or (diag(sign) . H)[perm][:, perm]  (H: Sylvester), M^T when `inverse`
+ * as an O(n log n) butterfly in `precision` (CT_F32, or CT_F64 for the fused weights), IEEE division by sqrt(n) in that precision,
+ * one conversion to `dtype` (fp64 reaches 16-bit dtypes through fp32, as torch's CPU conversion does).  x and out are [B, H, S, D]
+ * views with the same element strides (stride[3] == 1; anything else returns CT_E_UNSUPPORTED: run it on a contiguous copy); sign is
+ * int8 +-1 [n] or NULL, perm int64 [n] or NULL, both on the device of x.  device = CT_DEVICE_CPU runs the host twin (same butterfly
+ * order, same bits) on host pointers.  Enqueue-only on a device. */
+typedef struct ct_hadamard_job {
+    const void* x;
+    void* out;
+    int64_t shape[4];       /* B, H, S, D */
+    int64_t stride[4];      /* element strides of x and out */
+    const int8_t* sign;
+    const int64_t* perm;
+    int32_t dtype;          /* x and out: CT_F32 / CT_F16 / CT_BF16 */
+    int32_t precision;      /* CT_F32 / CT_F64 */
+    int32_t log2_n;
+    int32_t inverse;
+} ct_hadamard_job;
+int ct_hadamard_transform(const ct_hadamard_job* job, int device, void* stream);
 
 /* ---- fused compressor bodies ------------------------------------------------
  * quantize(dtype=int8) -> pack_to_int32 in one pass (pack_quantized/base.py:96-104) and

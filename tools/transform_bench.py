@@ -1,0 +1,120 @@
+#!/usr/bin/env python
+"""
+Walsh-Hadamard transforms on the H100: ops.hadamard_transform (ct_hadamard_transform) against the reference's dense formula on the same
+GPU (cast to fp32 -> matmul with the n x n matrix -> divide by sqrt(n) -> cast back), on Llama-3-8B shapes.
+
+    python tools/transform_bench.py [--iters 50] [--warmup 10] [--json out.json]
+
+Cases: online R1 on activations [8192, 4096] bf16 (n = 4096); R3 on q / k in the transposed [B, 32 | 8, S, 128] layout the attention
+hooks receive, prefill (B=1, S=8192) and decode (B=64, S=1); fp64 fusion (weight_input, n = 4096) of every 4096-input weight of the
+8B model (q, k, v, o, gate, up per layer: 32 layers, one layer's tensors reused).  Per case: time per call from CUDA events after
+warm-up, the algorithmic bandwidth (read + write of the tensor), its share of 3.35 TB/s and of the copy rate of tools/hbm_ceilings.py
+measured in the same run, the dense formula's time, and whether both outputs lie within the parity bound of DESIGN.md section 3.  The
+card, its power limit and max SM clock are printed with the numbers.
+"""
+import argparse
+import json
+import math
+import os
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from compressed_tensors_b200 import ops  # noqa: E402
+from compressed_tensors_b200.transform.utils.hadamard import deterministic_hadamard_matrix  # noqa: E402
+from tools.hbm_ceilings import rate  # noqa: E402
+
+HBM_PEAK = 3.35e12
+
+
+def card():
+    name = torch.cuda.get_device_name()
+    try:
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
+                               text=True, timeout=30).stdout.strip().splitlines()[torch.cuda.current_device()]
+    except Exception as e:  # noqa: BLE001 -- report, do not guess
+        power = f"unknown ({e})"
+    return name, power
+
+
+def timed(fn, iters, warmup):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) * 1e3 / iters
+
+
+def dense(x, w, precision):
+    """the reference's HadamardTransform formula, block-diagonal over the last dimension"""
+    n = w.shape[0]
+    y = x.to(precision).unflatten(-1, (-1, n)) @ w
+    return (y.flatten(-2) / torch.tensor(n, dtype=torch.float64).sqrt()).to(x.dtype)
+
+
+def within_bound(y, x, w):
+    """every element within (log2 n + 1) 2^-24 |x_row| of the float64 product, plus half an ulp of y's dtype"""
+    n = w.shape[0]
+    ref = (x.double().unflatten(-1, (-1, n)) @ w.double()) / math.sqrt(n)
+    err = (y.double().unflatten(-1, (-1, n)) - ref).abs()
+    half_ulp = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11, torch.float32: 0.0}[y.dtype]
+    bound = (math.log2(n) + 1) * 2.0 ** -24 * x.double().unflatten(-1, (-1, n)).norm(dim=-1, keepdim=True) + half_ulp * ref.abs()
+    return bool((err <= bound).all())
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--json")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("transform_bench needs a CUDA device")
+    gen = torch.Generator(device="cuda").manual_seed(0)
+    name, power = card()
+    n_copy = 1 << 30
+    src = torch.ones(n_copy, dtype=torch.bfloat16, device="cuda")
+    dst = torch.empty_like(src)
+    copy_gbs = rate(lambda: dst.copy_(src), n_copy * 4)
+    del src, dst
+    print(f"{name}, power limit / max SM clock: {power}; copy rate {copy_gbs} GB/s")
+
+    cases = []
+    x = torch.randn(8192, 4096, device="cuda", generator=gen).bfloat16()
+    cases.append(("R1 online [8192, 4096] bf16, n=4096", x, 4096, torch.float32))
+    for label, (B, H, S) in (("R3 q prefill [1, 32, 8192, 128]", (1, 32, 8192)), ("R3 k prefill [1, 8, 8192, 128]", (1, 8, 8192)),
+                             ("R3 q decode [64, 32, 1, 128]", (64, 32, 1)), ("R3 k decode [64, 8, 1, 128]", (64, 8, 1))):
+        cases.append((label, torch.randn(B, S, H, 128, device="cuda", generator=gen).bfloat16().transpose(1, 2), 128, torch.float32))
+    w = torch.randn(4096 + 1024 + 1024 + 4096 + 2 * 14336, 4096, device="cuda", generator=gen).bfloat16() * 0.02   # q, k, v, o, gate, up rows
+    cases.append(("fp64 fusion of one layer's 4096-input weights (x32 layers)", w, 4096, torch.float64))
+
+    results = []
+    for label, t, n, precision in cases:
+        h = deterministic_hadamard_matrix(n, precision, "cuda")
+        layers = 32 if precision == torch.float64 else 1
+        us = timed(lambda: ops.hadamard_transform(t, n, precision=precision), a.iters, a.warmup) * layers
+        us_dense = timed(lambda: dense(t, h, precision), max(3, a.iters // 5), 2) * layers
+        y = ops.hadamard_transform(t, n, precision=precision)
+        ok, ok_dense = within_bound(y, t, h), within_bound(dense(t, h, precision), t, h)
+        nbytes = t.numel() * t.element_size() * 2 * layers
+        gbs = nbytes / (us * 1e-6) / 1e9
+        r = dict(case=label, us=round(us, 1), gbs=round(gbs, 1), of_peak=round(gbs * 1e9 / HBM_PEAK, 3),
+                 of_copy=round(gbs / copy_gbs, 3), dense_us=round(us_dense, 1), speedup=round(us_dense / us, 2),
+                 kernel_within_bound=ok, dense_within_bound=ok_dense)
+        results.append(r)
+        print(json.dumps(r))
+    if a.json:
+        with open(a.json, "w") as f:
+            json.dump(dict(card=name, power=power, copy_gbs=copy_gbs, results=results), f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
