@@ -542,19 +542,24 @@ def _hadamard_job(x: torch.Tensor, out: torch.Tensor, log2_n: int, sign, perm, i
     return j
 
 
-def _check_permutation(perm: torch.Tensor, n: int) -> None:
-    """perm must be a permutation of 0 .. n-1 (the kernel scatters and gathers through it).  The values are checked once per version of
-    the tensor: callers that pass the same device copy every call (HadamardTransform) pay for one check."""
+def _verified_permutation(perm: torch.Tensor, n: int) -> torch.Tensor:
+    """perm must be a permutation of 0 .. n-1: the kernel scatters and gathers shared memory through it.  Returns an int64 copy made
+    when the values were checked, and the kernel reads only that copy.  The check runs once per version and storage of the tensor:
+    callers that pass the same tensor every call (HadamardTransform) pay for one check.  A write through `perm.data` changes neither,
+    as torch does not track it, so it is not seen; the copy keeps such a write from reaching the kernel unchecked."""
     if perm.dtype not in (torch.int64, torch.int32) or perm.ndim != 1 or perm.numel() != n:
         raise ValueError(f"perm must be a 1-D integer permutation of {n} indices, got shape {tuple(perm.shape)} and dtype {perm.dtype}")
     if perm.device.type == "meta":
-        return
+        return perm
     key = (perm._version, perm.data_ptr())
-    if getattr(perm, "_ct_checked_permutation", None) == key:
-        return
+    cached = getattr(perm, "_ct_checked_permutation", None)
+    if cached is not None and cached[0] == key:
+        return cached[1]
     if not torch.equal(torch.sort(perm).values, torch.arange(n, device=perm.device, dtype=perm.dtype)):
         raise ValueError(f"perm is not a permutation of 0 .. {n - 1}")
-    perm._ct_checked_permutation = key
+    checked = perm.detach().to(torch.int64, copy=True).contiguous()
+    perm._ct_checked_permutation = (key, checked)
+    return checked
 
 
 @torch.no_grad()
@@ -564,7 +569,9 @@ def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = N
     `(x.to(precision) @ M / sqrt(n)).to(x.dtype)` along the last dimension, block-diagonal over its n-element blocks, for the structured
     matrices of the `hadamard` / `random-hadamard` factories: M = H (Sylvester), with rows and columns permuted by `perm` (a permutation
     of 0 .. n-1) and / or rows signed by `sign` (n values, negative -> -1, else +1: diag(sign) . H); `inverse` applies M^T.  A `sign`
-    or `perm` of another length, or a `perm` that is not a permutation, raises ValueError.  An O(n log n) butterfly
+    or `perm` of another length, or a `perm` that is not a permutation, raises ValueError.  `perm` is checked once per version of the
+    tensor and the kernel uses the copy made at that check, so a write through `perm.data` (untracked by torch) is not seen until the
+    tensor's next tracked write.  An O(n log n) butterfly
     (ct_hadamard_transform) instead of the dense product; precision fp32 or fp64.  The output has x's strides when x is dense (the
     transposed [B, H, S, D] attention states included), so no contiguous copy is made in or out.
     """
@@ -581,7 +588,7 @@ def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = N
     if sign is not None and (sign.numel() != n or sign.dtype not in (torch.int8, torch.float32, torch.float64, torch.float16, torch.bfloat16)):
         raise ValueError(f"sign must hold {n} signs, got {sign.numel()} of dtype {sign.dtype}")
     if perm is not None:
-        _check_permutation(perm, n)
+        perm = _verified_permutation(perm, n)
     if x.device.type == "meta" or x.numel() == 0:
         return torch.empty_like(x)
     idx = _dev_index(x)
@@ -596,7 +603,7 @@ def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = N
         v = v.contiguous()
         out = torch.empty_like(v)
     sg = _to_dev(torch.where(sign < 0, -1, 1).to(torch.int8) if sign is not None and sign.dtype != torch.int8 else sign, idx)
-    pm = _to_dev(perm.to(torch.int64) if perm is not None else None, idx)
+    pm = _to_dev(perm, idx)
     log2_n = n.bit_length() - 1
     rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision)), idx, _stream(idx))
     if rc == N.CT_E_UNSUPPORTED and not v.is_contiguous():

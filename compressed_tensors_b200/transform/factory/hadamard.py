@@ -59,6 +59,17 @@ class HadamardFactory(TransformFactory):
 
 
 class HadamardTransform(TransformBase):
+    """
+    y = value . M / sqrt(n) with M = weight, or weight[perm][:, perm], transposed with `inverse`.
+
+    The kernel runs with copies of the signs Q and of `perm` made when they were verified.  Tracked writes (`copy_` and other
+    in-place ops, `load_state_dict`, `update_offload_parameter`, assigning `weight.data = t`) change the tensor's version or storage
+    and are seen on the next call.  In-place writes through `.data` (`weight.data.mul_(-1)`) are not: torch does not track them, and
+    re-verifying on every call would cost a host synchronisation per call.  After such a write the kernel path keeps computing with
+    the verified copies, while the dense path (an input that needs autograd, a trained weight, or a weight location the kernel does
+    not take) reads the live `weight` and `perm`, so the two paths can disagree until the next tracked write.
+    """
+
     _dynamic_tied_weights_keys: list[str] = ["weight", "perm"]
 
     def __init__(self, weight: Parameter, perm: Parameter | None, scheme: TransformScheme, args: TransformArgs,
@@ -123,14 +134,18 @@ def _structured_signs(weight: Tensor, perm: Tensor | None, value: Tensor):
     sign = _on(entry, value.device)
     if perm is None:
         return sign, None
-    pentry = _verified(perm, "_ct_hadamard_perm", lambda p: p if p.ndim == 1 and p.numel() == n and _is_permutation(p) else None)
+    pentry = _verified(perm, "_ct_hadamard_perm", lambda p: p.clone() if p.ndim == 1 and p.numel() == n and _is_permutation(p) else None)
     if pentry is None:
         return None
     return sign, _on(pentry, value.device)
 
 
 def _verified(t: Tensor, attr: str, check):
-    """check(t) once per version of `t`, kept on the tensor: (version, result on its own device, {device: copy})"""
+    """check(t) once per version of `t`, kept on the tensor: (version, data_ptr, result on its own device, {device: copy}).
+
+    `check` returns a snapshot that shares no memory with `t` (or True / None), and the kernel only ever receives that snapshot or
+    copies of it.  A write through `t.data` bumps neither key, so it is not seen until the next tracked write; until then the
+    transform keeps computing with the signs and permutation it verified, never with unverified indices."""
     cached = getattr(t, attr, None)
     if cached is None or cached[0] != t._version or cached[1] != t.data_ptr():
         with torch.no_grad():
@@ -165,7 +180,7 @@ def _sign_vector(w: Tensor):
         expected = (1 - 2 * (p & 1)).to(w.dtype) * q[r0:r0 + block, None]
         if not torch.equal(w[r0:r0 + block], expected):
             return None
-    return True if bool((q == 1).all()) else q.to(torch.int8).contiguous()
+    return True if bool((q == 1).all()) else q.to(torch.int8).contiguous()   # w is fp32 / fp64: .to(int8) is a copy
 
 
 def _is_permutation(p: Tensor) -> bool:

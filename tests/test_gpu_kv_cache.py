@@ -46,14 +46,18 @@ def qparams(x, args):
     return scale.to(x.dtype), (zp if not args.symmetric else None)
 
 
-def check_pair(xs, args, what=""):
-    sz = [qparams(x, args) for x in xs]
+def check_pair(xs, args, what="", sz=None):
+    """fake_quantize_heads of xs against fake_quantize and the oracle, with the qparams `sz` ([(scale, zero point)], default: the
+    observer's); returns the number of launches"""
+    sz = sz or [qparams(x, args) for x in xs]
     scales, zps = [s for s, _ in sz], [z for _, z in sz]
     n0 = N.launch_count()
     got = ops.fake_quantize_heads(xs, scales, zps, args)
     launches = N.launch_count() - n0
     for i, (x, g) in enumerate(zip(xs, got)):
-        assert g.stride() == x.stride() and g.dtype == x.dtype
+        assert g.shape == x.shape and g.stride() == x.stride() and g.dtype == x.dtype
+        if x.numel() == 0:
+            continue
         want = ops.fake_quantize(x.contiguous(), scales[i], zps[i], args)
         same(g, want, f"{what} tensor {i} vs fake_quantize: ")
         ref = oracle.fake_quantize(x.cpu(), scales[i].cpu(), zps[i].cpu() if zps[i] is not None else None, strategy=str(getattr(args.strategy, "value", args.strategy)),
@@ -62,7 +66,9 @@ def check_pair(xs, args, what=""):
     return launches
 
 
-SCHEMES = [("int", 8, True), ("int", 8, False), ("int", 4, True), ("int", 4, False), ("float", 8, True)]
+# int 2 .. 8 bits (bf16 at 7 bits is the last width of the narrow rounding, dispatch.cu), symmetric and asymmetric, and fp8
+SCHEMES = [("int", 8, True), ("int", 8, False), ("int", 4, True), ("int", 4, False), ("float", 8, True), ("int", 2, False), ("int", 3, True),
+           ("int", 5, False), ("int", 6, True), ("int", 7, True), ("int", 7, False)]
 LAYOUTS = [("contiguous", 2, 4, 16, 64), ("hf", 2, 4, 16, 64), ("hf", 3, 8, 5, 128), ("hf", 64, 8, 1, 128)]   # GQA heads, decode (S = 1)
 
 
@@ -78,6 +84,74 @@ def test_fake_quantize_heads_matches_fake_quantize_and_oracle(dtype, strategy, s
     assert check_pair([k, v], args) == 1        # one launch for the K / V pair
     q = hf_states(b, 2 * h, s, d, dtype, gen, lay)
     assert check_pair([q], args) == 1
+
+
+def _per_head(values, dtype, strategy):
+    """one value per head ([H, 1, 1], ATTN_HEAD) or the first one ([1], TENSOR)"""
+    t = torch.tensor(values, dtype=torch.float64).to(dtype).to(DEV)
+    return t.reshape(-1, 1, 1) if strategy == "attn_head" else t[:1]
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
+@pytest.mark.parametrize("strategy", ["tensor", "attn_head"])
+def test_fp8_with_the_all_zero_float8_zero_point(dtype, strategy):
+    """an FP8 KV scheme applied before compression registers an all-zero float8_e4m3fn zero point (initialize_qparams with
+    force_zero_point): the kernel's third zero-point kind"""
+    gen = torch.Generator().manual_seed(20)
+    args = qargs(strategy, "float", 8, True)
+    k, v = hf_states(2, 4, 16, 64, dtype, gen, "hf"), hf_states(2, 4, 16, 64, dtype, gen, "hf")
+    sz = []
+    for x in (k, v):
+        scale, _ = qparams(x, args)
+        sz.append((scale, torch.zeros(scale.shape, dtype=torch.float8_e4m3fn, device=DEV)))
+    assert check_pair([k, v], args, sz=sz) == 1
+
+
+@pytest.mark.parametrize("scheme", [("int", 8, False), ("float", 8, True)], ids=["int8a", "fp8"])
+@pytest.mark.parametrize("strategy", ["tensor", "attn_head"])
+def test_empty_key_and_unequal_pair(strategy, scheme):
+    """an empty K beside a non-empty V (the whole grid is V's), and K / V of different shapes whose chunk counts (of 8 elements)
+    are not multiples of the 1024 chunks of a block"""
+    gen = torch.Generator().manual_seed(21)
+    args = qargs(strategy, scheme[0], scheme[1], scheme[2])
+    v = hf_states(2, 4, 5, 64, torch.bfloat16, gen, "hf")
+    empty = hf_states(2, 4, 0, 64, torch.bfloat16, gen, "hf")
+    vsz = qparams(v, args)
+    assert check_pair([empty, v], args, sz=[vsz, vsz]) == 1
+    k = hf_states(1, 8, 37, 128, torch.bfloat16, gen, "hf")
+    assert (k.numel() // 8) % 1024 and (v.numel() // 8) % 1024
+    assert check_pair([k, v], args) == 1
+    assert check_pair([v, k], args) == 1
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("strategy", ["tensor", "attn_head"])
+@pytest.mark.parametrize("scheme", [("int", 8, True), ("int", 4, False), ("float", 8, True)], ids=["int8s", "int4a", "fp8"])
+def test_scales_outside_2_pow_100(dtype, strategy, scheme):
+    """scales of 2^-101 and 2^101 (per head: both, and 1), where x / scale is an IEEE division rather than a reciprocal product"""
+    gen = torch.Generator().manual_seed(22)
+    args = qargs(strategy, scheme[0], scheme[1], scheme[2])
+    qmax = 448.0 if scheme[0] == "float" else 2.0 ** (scheme[1] - 1)
+    for values in ([2.0 ** -101, 2.0 ** 101, 1.0, 2.0 ** -101], [2.0 ** 101, 2.0 ** -101, 2.0 ** -101, 1.0]):
+        scale = _per_head(values, dtype, strategy)
+        heads = scale.reshape(-1).double().cpu() if strategy == "attn_head" else scale.double().cpu().expand(4)
+        xs = [(torch.randn(2, 16, 4, 64, generator=gen, dtype=torch.float64) * heads.reshape(1, 1, 4, 1) * qmax / 3).to(dtype).to(DEV)
+              .transpose(1, 2) for _ in range(2)]
+        zp = None if scheme[2] else torch.randint(-3, 3, scale.shape, generator=gen, dtype=torch.int8).to(DEV)
+        assert check_pair(xs, args, sz=[(scale, zp), (scale, zp)]) == 1
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
+@pytest.mark.parametrize("scheme", [("int", 8, False), ("int", 4, True), ("float", 8, True)], ids=["int8a", "int4s", "fp8"])
+def test_infinite_inputs(dtype, scheme):
+    """+-inf states clamp to the ends of the grid as fake_quantize and the oracle clamp them"""
+    gen = torch.Generator().manual_seed(23)
+    for strategy in ("tensor", "attn_head"):
+        args = qargs(strategy, scheme[0], scheme[1], scheme[2])
+        k, v = hf_states(2, 4, 16, 64, dtype, gen, "hf"), hf_states(2, 4, 16, 64, dtype, gen, "hf")
+        sz = [qparams(x, args) for x in (k, v)]
+        k[0, 1, 3, 5], k[1, 3, 0, 63], v[0, 0, 0, 0], v[1, 2, 15, 8] = float("inf"), float("-inf"), float("-inf"), float("inf")
+        assert check_pair([k, v], args, sz=sz) == 1
 
 
 def test_llama3_8b_prefill_shape():

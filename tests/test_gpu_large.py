@@ -104,6 +104,44 @@ def test_nvfp4_pack_and_back(weights):
     _tiled_equal(ops.unpack_dequantize_fp4(packed, S, GS, dtype=torch.bfloat16), tile_back, "unpack_dequantize_fp4")
 
 
+def test_hadamard_transform(weights):
+    """rows of order 128 (signed, permuted) and 16384; the tile's output against the float64 reference"""
+    from tests.test_transform_host import assert_online_bound, structured_reference
+
+    tile, big = weights
+    g = torch.Generator().manual_seed(14)
+    for n, signed in ((128, True), (16384, False)):
+        q = (torch.randint(0, 2, (n,), generator=g) * 2 - 1).to(torch.int8).to(DEV) if signed else None
+        perm = torch.randperm(n, generator=g).to(DEV) if signed else None
+        tile_out = ops.hadamard_transform(tile.to(DEV), n, q, perm)
+        assert_online_bound(tile_out, structured_reference(tile.to(DEV), n, q, perm), tile.to(DEV), n)
+        _tiled_equal(ops.hadamard_transform(big, n, q, perm), tile_out, f"hadamard_transform n={n}")
+
+
+def test_attention_view_heads_and_hadamard(weights):
+    """the tensor as strided [B, H, S, D] attention states (B = REP, H = 16, S = 64, D = 1024): fake_quantize_heads per tensor and per
+    head against the oracle, and hadamard_transform along D"""
+    from tests.test_transform_host import assert_online_bound, structured_reference
+
+    tile, big = weights
+    view = big.view(REP, TILE_ROWS, 16, COLS // 16).transpose(1, 2)
+    tview = tile.to(DEV).view(1, TILE_ROWS, 16, COLS // 16).transpose(1, 2)
+    amax = tview.float().abs().amax((0, 2, 3))
+    for strategy, scale in (("tensor", (amax.max() / 127).reshape(1)), ("attn_head", (amax / 127).reshape(16, 1, 1))):
+        a = QuantizationArgs(num_bits=8, type="int", symmetric=True, strategy=strategy)
+        scale = scale.to(torch.bfloat16)
+        want = oracle.fake_quantize(tview.cpu(), scale.cpu(), None, strategy=strategy, num_bits=8, qtype="int").to(DEV)
+        (got,) = ops.fake_quantize_heads([view], [scale], [None], a)
+        assert got.stride() == view.stride()
+        _tiled_equal(got.transpose(1, 2).reshape(big.shape), want.transpose(1, 2).reshape(tile.shape), f"fake_quantize_heads {strategy}")
+        del got
+    tile_out = ops.hadamard_transform(tview, 1024)
+    assert_online_bound(tile_out, structured_reference(tview, 1024), tview, 1024)
+    out = ops.hadamard_transform(view, 1024)
+    assert out.stride() == view.stride()
+    _tiled_equal(out.transpose(1, 2).reshape(big.shape), tile_out.transpose(1, 2).reshape(tile.shape), "hadamard_transform [B, H, S, D]")
+
+
 def test_sparse_formats(weights):
     tile, big = weights
     v, m = ops.sparse24_compress(big)

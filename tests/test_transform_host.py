@@ -50,6 +50,59 @@ def assert_online_bound(y, ref, x, n):
     assert bool((err <= bound).all()), float((err - bound).max())
 
 
+def assert_fp64_result(y, ref, x, n):
+    """fp64 compute: 16-bit inputs give the float64 value rounded through fp32 (their sums are exact in float64), fp32 inputs lie within
+    half an fp32 ulp plus (log2 n + 1) 2^-53 |x_row| of it"""
+    if x.dtype != torch.float32:
+        assert torch.equal(y, ref.float().to(x.dtype)), int((y.double() != ref.float().to(x.dtype).double()).sum())
+        return
+    err = (y.double() - ref).abs().unflatten(-1, (-1, n))
+    row_norm = x.double().unflatten(-1, (-1, n)).norm(dim=-1, keepdim=True)
+    bound = (math.log2(n) + 1) * 2.0 ** -53 * row_norm + 2.0 ** -24 * ref.abs().unflatten(-1, (-1, n))
+    assert bool((err <= bound).all()), float((err - bound).max())
+
+
+def fwht64(z):
+    """z . H_n along the last dimension in float64 (n its length, a power of two), by recursive halves:
+    (a, b) . H_2m = ((a + b) . H_m, (a - b) . H_m), the halves taken first (the kernel pairs neighbours first)"""
+    z = z.double()
+    h = z.shape[-1] // 2
+    while h >= 1:
+        v = z.unflatten(-1, (-1, 2, h))
+        z = torch.stack((v[..., 0, :] + v[..., 1, :], v[..., 0, :] - v[..., 1, :]), -2).flatten(-3)
+        h //= 2
+    return z
+
+
+def structured_matrix(n, sign=None, perm=None, inverse=False):
+    """the dense M of hadamard.cu's header, from its definition: (diag(Q) . H)[perm][:, perm], transposed for the inverse;
+    H is scipy's Sylvester matrix"""
+    import scipy.linalg
+
+    m = torch.from_numpy(scipy.linalg.hadamard(n).astype("float64"))
+    if sign is not None:
+        m = torch.where(sign < 0, -1.0, 1.0).double().unsqueeze(1) * m
+    if perm is not None:
+        m = m[perm][:, perm]
+    return m.T if inverse else m
+
+
+def structured_reference(x, n, sign=None, perm=None, inverse=False):
+    """float64 x . M / sqrt(n), block-diagonal over the last dimension, for every order through fwht64.  With p = perm and Q = sign,
+    M[i][j] = Q[p[i]] H[p[i]][p[j]], so y[j] = (z . H)[p[j]] with z[p[i]] = Q[p[i]] x[i]; M^T[i][j] = Q[p[j]] H[p[j]][p[i]], so
+    y[j] = Q[p[j]] (z . H)[p[j]] with z[p[i]] = x[i].  test_fwht_reference_equals_dense_product checks this against
+    structured_matrix.  Runs on x's device (plain float64 additions, the same on every device)."""
+    xb = x.double().unflatten(-1, (-1, n))
+    q = torch.ones(n, dtype=torch.float64, device=x.device) if sign is None else torch.where(sign.to(x.device) < 0, -1.0, 1.0).double()
+    p = torch.arange(n, device=x.device) if perm is None else perm.to(x.device)
+    z = torch.empty_like(xb)
+    z[..., p] = xb if inverse else xb * q[p]
+    y = fwht64(z)[..., p]
+    if inverse:
+        y = y * q[p]
+    return y.flatten(-2) / math.sqrt(n)
+
+
 def _case_id(c):
     return f"{c['type']}-{'rand' if c['randomize'] else 'fixed'}-{c['location']}-hd{c['head_dim']}-{c['dtype'].split('.')[-1]}"
 
@@ -85,23 +138,39 @@ def test_factory_golden(case, eager):
                 assert torch.equal(tfm(module.bias.unsqueeze(-1)).squeeze(-1), case["fused_bias"])
 
 
+def transform_cases(n, gen):
+    """(sign, perm, inverse) for the four structured forms and their transposes"""
+    q = (torch.randint(0, 2, (n,), generator=gen) * 2 - 1).to(torch.int8)
+    perm = torch.randperm(n, generator=gen)
+    return [(s, p, inv) for s in (None, q) for p in (None, perm) for inv in (False, True)]
+
+
+def test_fwht_reference_equals_dense_product():
+    """structured_reference (recursive halves) against x . M with M built densely from scipy's Sylvester matrix, bit for bit on
+    bf16-valued inputs (their float64 sums are exact, so the two summation orders agree)"""
+    gen = torch.Generator().manual_seed(1)
+    for log2_n in range(1, 13):
+        n = 1 << log2_n
+        x = torch.randn(3, 2 * n, generator=gen).bfloat16()
+        for sign, p, inverse in transform_cases(n, gen):
+            m = structured_matrix(n, sign, p, inverse)
+            if sign is None and p is None:
+                assert torch.equal(m, deterministic_hadamard_matrix(n, torch.float64))
+            dense = (x.double().unflatten(-1, (-1, n)) @ m).flatten(-2) / math.sqrt(n)
+            assert torch.equal(structured_reference(x, n, sign, p, inverse), dense), (n, sign is None, p is None, inverse)
+
+
 def test_cpu_twin_matches_dense_product_for_every_form():
-    """the four structured forms and their transposes, against the dense matrix the factories build"""
+    """every order 2^1 .. 2^15, dtype, precision, the four structured forms and their transposes, against the float64 reference"""
     gen = torch.Generator().manual_seed(0)
-    for n in (2, 8, 64, 256):
-        x = torch.randn(3, 2 * n, generator=gen)
-        q = (torch.randint(0, 2, (n,), generator=gen) * 2 - 1).to(torch.int8)
-        perm = torch.randperm(n, generator=gen)
-        for sign in (None, q):
-            for p in (None, perm):
-                w = deterministic_hadamard_matrix(n, torch.float64)
-                if sign is not None:
-                    w = sign.double().unsqueeze(1) * w
-                for inverse in (False, True):
-                    ref = dense_reference(w, p, x, inverse)
-                    y64 = _eager(x.bfloat16(), n, sign, p, inverse, torch.float64)
-                    assert torch.equal(y64, dense_reference(w, p, x.bfloat16(), inverse).float().bfloat16())
-                    assert_online_bound(_eager(x, n, sign, p, inverse, torch.float32), ref, x, n)
+    for log2_n in range(1, 16):
+        n = 1 << log2_n
+        for dtype in (torch.bfloat16, torch.float16, torch.float32):
+            x = torch.randn(3 if n <= 4096 else 1, 2 * n, generator=gen).to(dtype)
+            for sign, p, inverse in transform_cases(n, gen):
+                ref = structured_reference(x, n, sign, p, inverse)
+                assert_fp64_result(_eager(x, n, sign, p, inverse, torch.float64), ref, x, n)
+                assert_online_bound(_eager(x, n, sign, p, inverse, torch.float32), ref, x, n)
 
 
 def _eager(*args):
@@ -176,6 +245,76 @@ def test_non_hadamard_weight_takes_the_dense_formula(eager):
         tfm.weight.mul_(0.5)
         tfm.weight[3, 5] = 0.25
     assert torch.equal(tfm(x), tfm._dense(x))
+
+
+def _random_hadamard_transform(device):
+    module = torch.nn.Linear(64, 64).to(device)
+    return TransformFactory.from_scheme(TransformScheme(type="random-hadamard", randomize=True), name="", seed=7).create_transform(
+        module, TransformArgs(targets="Linear", location="input"))
+
+
+def check_tracked_writes_are_followed(device):
+    """a new signed Hadamard weight and permutation written by copy_, load_state_dict, update_offload_parameter or assignment to
+    .data is what the next call computes with"""
+    from compressed_tensors_b200.offload import update_offload_parameter
+
+    gen = torch.Generator().manual_seed(8)
+    x = torch.randn(4, 64, generator=gen).to(device)
+    for write in ("copy_", "load_state_dict", "update_offload_parameter", "assign .data"):
+        t = _random_hadamard_transform(device)
+        before = t(x)
+        q = (torch.randint(0, 2, (64,), generator=gen) * 2 - 1).to(torch.int8).to(device)
+        perm = torch.randperm(64, generator=gen).to(device)
+        weight = q.to(t.weight.dtype).unsqueeze(1) * deterministic_hadamard_matrix(64, t.weight.dtype, device)
+        if write == "copy_":
+            with torch.no_grad():
+                t.weight.copy_(weight)
+                t.perm.copy_(perm)
+        elif write == "load_state_dict":
+            t.load_state_dict({"weight": weight, "perm": perm})
+        elif write == "update_offload_parameter":
+            update_offload_parameter(t, "weight", weight)
+            update_offload_parameter(t, "perm", perm)
+        else:
+            t.weight.data = weight
+            t.perm.data = perm
+        y = t(x)
+        assert not torch.equal(y, before), write
+        assert torch.equal(y, ops.hadamard_transform(x, 64, q, perm)), write
+        assert_online_bound(y.cpu(), structured_reference(x.cpu(), 64, q, perm), x.cpu(), 64)
+
+
+def check_data_writes_keep_the_verified_snapshot(device):
+    """in-place writes through .data are not tracked: the transform keeps computing with the signs and permutation it verified, never
+    with the stale signs and the live permutation; the next tracked write brings both up to date"""
+    gen = torch.Generator().manual_seed(9)
+    x = torch.randn(4, 64, generator=gen).to(device)
+    t = _random_hadamard_transform(device)
+    before = t(x)
+    q = t.weight[:, 0].detach().clone()
+    other = torch.randperm(64, generator=gen).to(device)
+    t.weight.data.mul_(-1)                  # diag(-Q) . H: still a signed Hadamard matrix
+    t.perm.data.copy_(other)                # still a permutation
+    assert torch.equal(t(x), before)
+    with torch.no_grad():
+        t.weight.mul_(1)
+        t.perm.add_(0)
+    assert torch.equal(t(x), ops.hadamard_transform(x, 64, -q, other))
+    # the op on its own: the permutation it checked, not one written through .data afterwards
+    perm = torch.randperm(64, generator=gen).to(device)
+    y = ops.hadamard_transform(x, 64, None, perm)
+    perm.data.copy_(torch.randperm(64, generator=gen).to(device))
+    assert torch.equal(ops.hadamard_transform(x, 64, None, perm), y)
+    perm.add_(0)
+    assert not torch.equal(ops.hadamard_transform(x, 64, None, perm), y)
+
+
+def test_tracked_writes_are_followed(eager):
+    check_tracked_writes_are_followed("cpu")
+
+
+def test_data_writes_keep_the_verified_snapshot(eager):
+    check_data_writes_keep_the_verified_snapshot("cpu")
 
 
 def _model_id(c):

@@ -152,6 +152,53 @@ def batched_family(dt):
     ops.batched(N.OP_SPARSE24_UNPACK_DEQUANTIZE, d24, 0)
 
 
+def transform_family(dt):
+    """ct_hadamard_transform: every order in both precisions with one-row partial last tiles, fp64 at 2^15 on more tiles than its
+    grid of 2 x SMs (CTAs reuse their global scratch slice), rows one element off alignment (element loads and stores) with sign,
+    perm and inverse, and strided [B, H, S, D] views with head blocking and decode"""
+    sms = torch.cuda.get_device_properties(DEV).multi_processor_count
+    for log2_n in range(1, 16):
+        n = 1 << log2_n
+        rows = 2 * sms + 7 if log2_n == 15 else (4096 // n + 1 if n < 4096 else 3)
+        x = torch.randn(rows, n, device=DEV).to(dt)
+        q = (torch.randint(0, 2, (n,), device=DEV) * 2 - 1).to(torch.int8)
+        perm = torch.randperm(n, device=DEV)
+        odd = torch.randn(3 * n + 1, device=DEV).to(dt)[1:].view(3, n) if n in (2, 16, 128, 4096) else None
+        for precision in (torch.float32, torch.float64):
+            for sign, p, inverse in ((None, None, False), (q, perm, False), (q, perm, True)):
+                ops.hadamard_transform(x, n, sign, p, inverse, precision)
+                if odd is not None:
+                    ops.hadamard_transform(odd, n, sign, p, inverse, precision)
+    for B, H, S, D, n in ((2, 8, 33, 64, 64), (2, 4, 17, 256, 64), (3, 8, 1, 256, 64), (1, 32, 256, 128, 128)):
+        x = torch.randn(B, S, H, D, device=DEV).to(dt).transpose(1, 2)
+        q = (torch.randint(0, 2, (n,), device=DEV) * 2 - 1).to(torch.int8)
+        for precision in (torch.float32, torch.float64):
+            ops.hadamard_transform(x, n, q, torch.randperm(n, device=DEV), True, precision)
+
+
+def heads_family(dt):
+    """ct_fake_quantize_heads: every zero-point kind (none, int8, all-zero float8) and rounding width, per tensor and per head, on
+    K / V pairs of unequal shapes, with an empty first job, and on one tensor"""
+    k = torch.randn(1, 37, 8, 128, device=DEV).to(dt).transpose(1, 2)
+    v = torch.randn(2, 5, 4, 64, device=DEV).to(dt).transpose(1, 2)
+    empty = torch.randn(2, 0, 4, 64, device=DEV).to(dt).transpose(1, 2)
+    schemes = [(8, "int", True, None), (8, "int", False, torch.int8), (7, "int", True, None), (4, "int", False, torch.int8),
+               (2, "int", True, None), (8, "float", True, None), (8, "float", True, torch.float8_e4m3fn)]
+    for strategy in ("tensor", "attn_head"):
+        for bits, qtype, sym, zdt in schemes:
+            a = qa(num_bits=bits, type=qtype, strategy=strategy, symmetric=sym)
+
+            def qp(x):
+                shape = (x.shape[1], 1, 1) if strategy == "attn_head" else (1,)
+                s = ((torch.rand(shape, device=DEV) + 0.1) / 2 ** (bits - 1)).to(dt)
+                z = None if zdt is None else (torch.randint(-2, 2, shape, device=DEV, dtype=torch.int8) if zdt == torch.int8
+                                              else torch.zeros(shape, device=DEV, dtype=zdt))
+                return s, z
+            for pair in ((k, v), (v, k), (empty, v), (k,)):
+                sz = [qp(x) for x in pair]
+                ops.fake_quantize_heads(list(pair), [s for s, _ in sz], [z for _, z in sz], a)
+
+
 FAILED = []
 
 
@@ -174,6 +221,8 @@ def main():
             attempt(sparse_family, rows, cols, dt)
             if dt != torch.float32:
                 attempt(observer_family, rows, cols, dt)
+        attempt(transform_family, dt)
+        attempt(heads_family, dt)
         torch.cuda.synchronize()
         print(f"{dt}: launches so far {N.launch_count()}", flush=True)
     for rows, cols in ((128, 128), (200, 384), (1024, 2048)):
