@@ -40,6 +40,7 @@ SOURCES = [
     "observe_tensor.cu",
     "cpu_twin.cu",
     "fast_observe.cu",
+    "dynamic_fake.cu",
 ]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + ["../../include/ct_b200.h"]   # every header: a stale object is a silent wrong build
 

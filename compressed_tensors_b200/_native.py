@@ -145,6 +145,7 @@ _PROTOS = {
     "ct_observe_quantize_channel": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_observe_tensor": (_int, [_descp, _vp, _int, _vp, _vp, _int, _vp]),
     "ct_observe_quantize_tensor": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),
+    "ct_dynamic_fake_quantize": (_int, [_descp, _int, _int, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_batched": (_int, [_int, _int, _descp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_pack_bitmasks": (_int, [_vp, _vp, _i64, _i64, _int, _vp]),
     "ct_unpack_bitmasks": (_int, [_vp, _vp, _i64, _i64, _int, _vp]),

@@ -10,12 +10,10 @@
 // computed redundantly by every lane of the group with the reference's per-op rounding to the weight
 // dtype T, and lane 0 of the group stores them.
 #include "engine.h"
+#include "observe_core.cuh"
 #include "ops.cuh"
 
 namespace ctb {
-
-template <class P> __device__ __forceinline__ float round_to_t(float v) { return P::lo(P::pack(v, 0.f)); }
-template <class P> __device__ __forceinline__ float eps_of() { return P::DT == CT_BF16 ? 0.0078125f : 0.0009765625f; }
 
 template <class P, int BITS, int ASYM, int LPG>
 struct ObserveQuantPackOp {
@@ -47,18 +45,8 @@ struct ObserveQuantPackOp {
         float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);   // max(max_vals, 0)
 
         // ---- calculate_qparams, each op rounded to T (helpers.py:74-131) ----
-        const float range = cm.qmax - cm.qmin;
-        float s, zq = 0.f;
-        if (ASYM) {
-            s = round_to_t<P>(__fdiv_rn(round_to_t<P>(__fsub_rn(hi, lo)), range));
-            float z = round_to_t<P>(__fsub_rn(cm.qmin, round_to_t<P>(__fdiv_rn(lo, s))));
-            z = clamp_nan(z, cm.qmin, cm.qmax);
-            z = clamp_nan(z, -128.f, 127.f);
-            zq = (z != z) ? 0.f : rintf(z);                        // round(...).to(int8); NaN (0/0) -> 0
-        } else {
-            s = round_to_t<P>(__fdiv_rn(fmaxf(fabsf(lo), fabsf(hi)), range * 0.5f));
-        }
-        if (s == 0.f) s = eps_of<P>();
+        float zq;
+        const float s = obs_scale_zp<P::DT>(lo, hi, ASYM, cm.qmin, cm.qmax, zq);
 
         const uint32_t gi = fd_div(gc0, J.dc);
         if ((threadIdx.x & (LPG - 1)) == 0) {

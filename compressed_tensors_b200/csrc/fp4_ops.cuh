@@ -10,6 +10,7 @@
 // adding +0.0f first.
 #pragma once
 
+#include "observe_core.cuh"
 #include "ops.cuh"
 
 namespace ctb {
@@ -231,13 +232,7 @@ struct Fp4NvObserveQuantPackOp {
     template <bool DIV>
     __device__ static __forceinline__ float group_scale(float amax, float gs, uint32_t& byte) {
         const float q6 = DIV ? __fdiv_rn(amax, 6.0f) : recip_div(amax, 6.0f, 0.16666667163372039794921875f);   // max_val_pos / (bit_range / 2)
-        const float st = P::lo(P::pack(q6, 0.f));                                                                  // ... in T
-        float sf = fminf(fmaxf(__fmul_rn(gs, st), -448.0f), 448.0f);             // global_scale * scales (float32), clamp
-        byte = f32x2_to_e4m3x2(sf, 0.f) & 0xffu;                                  // .to(float8_e4m3fn)
-        sf = e4m3_to_f32(byte);
-        if (sf == 0.f) { sf = 0.125f; byte = 0x20u; }                             // eps of the scale dtype; 0x20 = 0.125 in e4m3
-        if (sf != sf) byte = 0x7fu;
-        return sf;
+        return obs_fp8_scale(__fmul_rn(gs, obs_round<P::DT>(q6)), byte);          // ... in T, x global_scale (float32), as e4m3
     }
     struct SlowOut {
         uint4 nibbles;

@@ -9,6 +9,7 @@
 #include <cstring>
 
 #include "engine.h"
+#include "observe_core.cuh"
 #include "ops.cuh"
 
 namespace ctb {
@@ -16,8 +17,6 @@ namespace ctb {
 enum ChanOut { CO_PACK4 = 0, CO_PACK8 = 1, CO_I8 = 2, CO_F8 = 3 };
 constexpr int CH_MAXU = 8;   // most units (of 8 elements) per thread: rows up to 16384 columns.  The kernel is instantiated for 2, 4 and
                              // 8 units so that short rows do not pay for registers they do not use (more CTAs resident per SM)
-
-template <class P> __device__ __forceinline__ float ch_round_to_t(float v) { return P::lo(P::pack(v, 0.f)); }
 
 template <class P, int OUT, int ASYM, int MAXU>
 __global__ void __launch_bounds__(256) observe_channel_kernel(const uint4* __restrict__ x, void* __restrict__ scale_out, int8_t* __restrict__ zp_out,
@@ -50,18 +49,8 @@ __global__ void __launch_bounds__(256) observe_channel_kernel(const uint4* __res
         const float lo = fminf(fminf(P::lo(mn2), P::hi(mn2)), 0.f);   // min(min_vals, 0)
         const float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);   // max(max_vals, 0)
         // calculate_qparams, each op rounded to T (helpers.py:74-131)
-        const float range = cm.qmax - cm.qmin;
-        float s, zq = 0.f;
-        if (ASYM) {
-            s = ch_round_to_t<P>(__fdiv_rn(ch_round_to_t<P>(__fsub_rn(hi, lo)), range));
-            float z = ch_round_to_t<P>(__fsub_rn(cm.qmin, ch_round_to_t<P>(__fdiv_rn(lo, s))));
-            z = clamp_nan(z, cm.qmin, cm.qmax);
-            z = clamp_nan(z, -128.f, 127.f);
-            zq = (z != z) ? 0.f : rintf(z);
-        } else {
-            s = ch_round_to_t<P>(__fdiv_rn(fmaxf(fabsf(lo), fabsf(hi)), range * 0.5f));
-        }
-        if (s == 0.f) s = (P::DT == CT_BF16) ? 0.0078125f : 0.0009765625f;   // torch.finfo(T).eps
+        float zq;
+        const float s = obs_scale_zp<P::DT>(lo, hi, ASYM, cm.qmin, cm.qmax, zq);
         reinterpret_cast<unsigned short*>(scale_out)[r] = (unsigned short)P::from_float1(s);
         if (ASYM) zp_out[r] = (int8_t)(int)zq;
         qp[0] = s; qp[1] = zq;

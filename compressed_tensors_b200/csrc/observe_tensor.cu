@@ -13,6 +13,7 @@
 #include <cstring>
 
 #include "engine.h"
+#include "observe_core.cuh"
 #include "ops.cuh"
 
 namespace ctb {
@@ -35,13 +36,6 @@ __device__ __forceinline__ uint64_t l2_policy(bool keep) {
     else asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
     return p;
 }
-
-template <class P> __device__ __forceinline__ float to_t(float v) {
-    if constexpr (P::DT == CT_F32) return v;
-    else return P::lo(P::pack(v, 0.f));
-}
-template <class P> __device__ __forceinline__ float eps_t() { return P::DT == CT_BF16 ? 0.0078125f : (P::DT == CT_F16 ? 0.0009765625f : 1.1920928955078125e-07f); }
-template <class P> __device__ __forceinline__ float tiny_t() { return P::DT == CT_F16 ? 6.103515625e-05f : 1.1754943508222875e-38f; }
 
 struct ObsParams {
     float qmin, qmax;
@@ -106,25 +100,15 @@ __global__ void __launch_bounds__(256) minmax_qparams_kernel(const uint4* __rest
         // generate_gparam (helpers.py:308-337): 448 * 6 / clamp(max|x|, tiny) in x's dtype, NaN / inf -> 1, as float32.
         // `python_float / tensor` is Tensor.__rtruediv__ = tensor.reciprocal() * python_float: TWO roundings to x's dtype (1 / top, then
         // the product), not one division -- 2688 / 1.745 is 1541 in fp16 this way, 1540 by a correctly rounded quotient.
-        float top = fmaxf(fmaxf(fabsf(lo), fabsf(hi)), tiny_t<P>());
-        float g = to_t<P>(__fmul_rn(to_t<P>(__frcp_rn(top)), 2688.0f));
+        float top = fmaxf(fmaxf(fabsf(lo), fabsf(hi)), obs_tiny<P::DT>());
+        float g = obs_round<P::DT>(__fmul_rn(obs_round<P::DT>(__frcp_rn(top)), 2688.0f));
         if (g != g || fabsf(g) == __int_as_float(0x7f800000)) g = 1.0f;
         *reinterpret_cast<float*>(scale_out) = g;
         return;
     }
     // calculate_qparams, each op rounded to T (helpers.py:74-131)
-    const float range = prm.qmax - prm.qmin;
-    float s, zq = 0.f;
-    if (prm.asym) {
-        s = to_t<P>(__fdiv_rn(to_t<P>(__fsub_rn(hi, lo)), range));
-        float z = to_t<P>(__fsub_rn(prm.qmin, to_t<P>(__fdiv_rn(lo, s))));
-        z = clamp_nan(z, prm.qmin, prm.qmax);
-        z = clamp_nan(z, -128.f, 127.f);
-        zq = (z != z) ? 0.f : rintf(z);
-    } else {
-        s = to_t<P>(__fdiv_rn(fmaxf(fabsf(lo), fabsf(hi)), range * 0.5f));
-    }
-    if (s == 0.f) s = eps_t<P>();
+    float zq;
+    const float s = obs_scale_zp<P::DT>(lo, hi, prm.asym != 0, prm.qmin, prm.qmax, zq);
     if constexpr (P::DT == CT_F32) *reinterpret_cast<float*>(scale_out) = s;
     else *reinterpret_cast<unsigned short*>(scale_out) = (unsigned short)P::from_float1(s);
     if (prm.asym && zp_out) *zp_out = (int8_t)(int)zq;

@@ -34,6 +34,7 @@ __all__ = [
     "dequantize",
     "fake_quantize",
     "fake_quantize_heads",
+    "dynamic_fake_quantize",
     "hadamard_transform",
     "quantize_pack",
     "unpack_dequantize",
@@ -521,6 +522,82 @@ def fake_quantize_heads(tensors: Sequence[torch.Tensor], scales: Sequence[torch.
                 N.check(rc, "ct_fake_quantize_heads")
                 return outs
     return [fake_quantize(x, s, z, args) for x, s, z in zip(tensors, scales, zero_points)]
+
+
+# args.scale_dtype -> how the library rounds a fresh scale (CT_NONE: it stays in x's dtype)
+_SCALE_ROUNDING = {None: N.DT_NONE, torch.float8_e4m3fn: N.DT[torch.float8_e4m3fn], torch.uint8: N.DT_E8M0}
+_DYNAMIC_ZP_DTYPES = (torch.int8, torch.float8_e4m3fn, torch.uint8)
+
+
+def _dynamic_layout(x: torch.Tensor, args):
+    """(rows, cols, rdiv, cdiv, s_row_stride, scale shape) of compute_dynamic_scales_and_zp's reduction (utils/helpers.py:140-195),
+    or None for a strategy or shape the fused kernel does not take.  TOKEN reduces over every dim after the first two, so a 1-D or
+    2-D value reduces over the whole tensor, as the reference's aminmax does, and gets one scale."""
+    strategy, cols = _strategy_name(args), x.shape[-1]
+    if strategy == "token" and x.ndim > 2:
+        rows = x.shape[0] * x.shape[1]
+        return rows, x.numel() // rows, 1, N.INF, 1, tuple(x.shape[:2]) + (1,) * (x.ndim - 2)
+    if strategy in ("token", "tensor"):
+        return x.numel() // cols, cols, N.INF, N.INF, 0, (1,)
+    if strategy in ("group", "tensor_group"):
+        g = int(getattr(args, "group_size", 0) or 0)
+        if g <= 0 or cols % g != 0:
+            return None   # the reference's unflatten raises for a ragged last group: the two-step path raises it
+        return x.numel() // cols, cols, 1, g, cols // g, tuple(x.shape[:-1]) + (cols // g,)
+    return None
+
+
+@torch.no_grad()
+def dynamic_fake_quantize(x: torch.Tensor, args, global_scale: Optional[torch.Tensor] = None):
+    """
+    compute_dynamic_scales_and_zp (utils/helpers.py:140-195) followed by fake_quantize (forward.py:148-181) in one pass over x on
+    its GPU (`ct_dynamic_fake_quantize`): returns (out, scale, zero_point), the scale and zero point with the shapes and dtypes the
+    reference's compute_dynamic_scales_and_zp returns and `out` equal bit for bit to fake_quantize with them.
+    Returns None when the kernel does not take the input -- a CPU, non-contiguous or fp32 tensor, a last dimension not divisible by
+    8, a strategy, scheme or group size it does not cover -- and the caller then runs the two steps, which also raise whatever the
+    reference raises for the input.
+    """
+    if not x.is_cuda or not x.is_contiguous() or x.dtype not in (torch.bfloat16, torch.float16) or x.ndim == 0 or x.numel() == 0:
+        return None
+    if x.shape[-1] % 8 != 0 or getattr(_mode, "cpu", False):
+        return None
+    try:
+        qtype, bits = _qparams(args)
+    except (NotImplementedError, ValueError):
+        return None
+    layout = _dynamic_layout(x, args)
+    scale_dtype_arg = getattr(args, "scale_dtype", None)
+    zp_dtype = getattr(args, "zp_dtype", None)
+    if layout is None or scale_dtype_arg not in _SCALE_ROUNDING or zp_dtype not in _DYNAMIC_ZP_DTYPES:
+        return None
+    rows, cols, rdiv, cdiv, srs, scale_shape = layout
+    gs = None
+    scale_dtype = x.dtype
+    if global_scale is not None:
+        # `global_scale * scales` (helpers.py:93-94): a float32 [1] global scale promotes the scale to float32
+        if global_scale.dtype != torch.float32 or global_scale.numel() != 1 or global_scale.ndim == 0 or global_scale.device != x.device:
+            return None
+        gs = global_scale.reshape(1).contiguous()
+        scale_dtype = torch.float32
+    se = scale_dtype   # the effective scale dtype and compute dtype fake_quantize derives from that scale (ops.fake_quantize)
+    cd = torch.promote_types(x.dtype, se)
+    out = torch.empty_like(x)
+    scale = torch.empty(scale_shape, dtype=scale_dtype, device=x.device)
+    zero_point = torch.empty(scale_shape, dtype=zp_dtype, device=x.device)
+    d = N.QuantDesc()
+    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, rdiv, cdiv, srs
+    d.x_dtype = d.out_dtype = N.DT[x.dtype]
+    d.scale_dtype, d.zp_dtype, d.compute_dtype, d.seff_dtype = N.DT[scale_dtype], N.DT[zp_dtype], N.DT[cd], N.DT[se]
+    d.q_dtype, d.qtype, d.num_bits = N.DT_NONE, qtype, bits
+    d.global_scale = gs.data_ptr() if gs is not None else None
+    d.aux = None
+    idx = x.get_device()
+    rc = N.lib().ct_dynamic_fake_quantize(ctypes.byref(d), int(not args.symmetric), _SCALE_ROUNDING[scale_dtype_arg], N.ptr(x), N.ptr(out),
+                                          N.ptr(scale), N.ptr(zero_point), idx, N.stream_ptr(idx))
+    if rc == N.CT_E_UNSUPPORTED:
+        return None
+    N.check(rc, "ct_dynamic_fake_quantize")
+    return out, scale, zero_point
 
 
 # --------------------------------------------------------------------------------------------

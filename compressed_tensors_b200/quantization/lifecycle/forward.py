@@ -66,6 +66,12 @@ def forward_quantize(module: Module, value: torch.Tensor, base_name: str, args: 
     g_idx = getattr(module, "weight_g_idx", None)
     global_scale = getattr(module, f"{base_name}_global_scale", None)
     if args.dynamic in (True, DynamicType.LOCAL):
+        # observer and fake quantization in one pass on the device (bit-identical); CPU, strided or g_idx inputs and whatever the kernel
+        # declines take the two steps below, so their results and errors are the reference's
+        if g_idx is None and value.is_cuda and value.is_contiguous():
+            fused = ops.dynamic_fake_quantize(value, args, global_scale=global_scale)
+            if fused is not None:
+                return fused[0]
         scale, zero_point = compute_dynamic_scales_and_zp(value=value, args=args, module=module, global_scale=global_scale)
     else:
         scale = getattr(module, f"{base_name}_scale")

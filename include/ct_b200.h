@@ -255,6 +255,26 @@ int ct_observe_quantize_channel(const ct_quant_desc* d, const void* x, void* sca
 int ct_observe_tensor(const ct_quant_desc* d, const void* x, int kind, void* scale_out, void* zp_out, int device, void* stream);
 int ct_observe_quantize_tensor(const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, void* q_out, int device, void* stream);
 
+/* ---- dynamic activation quantization in one pass ---------------------------------------------------
+ * replaces compute_dynamic_scales_and_zp (quantization/utils/helpers.py:140-195) followed by fake_quantize (forward.py:148-181), the
+ * dynamic branch of forward_quantize (forward.py:292-329): the memoryless min-max observer and calculate_qparams (helpers.py:50-137)
+ * fused with quantize-dequantize, so x [rows, cols] (bf16 / fp16, contiguous, cols % 8 == 0, 16-byte aligned) is read once.
+ *   out        x's shape and dtype: the fake-quantized values, bit-identical to ct_fake_quantize with the qparams below
+ *   scale_out  x's dtype, or float32 when d->global_scale is given (NVFP4: global_scale * scales promotes); zp_out d->zp_dtype
+ *              (CT_I8, CT_F8E4M3 or CT_U8, zeros for a symmetric scheme); one element per row / group / tensor
+ * The strategy is read from the scale addressing of d:
+ *   TOKEN   rdiv = 1, s_row_stride = 1, cdiv = CT_DIV_INF: one scale per row (the caller folds every dim after the first two into cols),
+ *           cols <= 32768; int (asymmetric: int8 zero point) or fp8
+ *   GROUP   rdiv = 1, cdiv = group size in {16, 32, 64, 128} dividing cols, s_row_stride = cols / cdiv (also TENSOR_GROUP)
+ *   TENSOR  rdiv = cdiv = CT_DIV_INF: ct_observe_tensor (kind 0), then ct_fake_quantize on the device-resident scale
+ * asymmetric: args.symmetric is False.  scale_dtype_arg: args.scale_dtype as CT_NONE, CT_F8E4M3 (clamp to +-448 and round through
+ * float8_e4m3fn, optionally after d->global_scale, a DEVICE pointer to one float32) or CT_E8M0 (uint8: the MX exponent scales of
+ * generate_mx_scales / maybe_convert_from_mx_exp, quantization/utils/mxfp_utils.py:47-139, group 32).  d->compute_dtype / d->seff_dtype
+ * are those ct_fake_quantize would get for the returned scale.  Anything else, and device = CT_DEVICE_CPU, returns CT_E_UNSUPPORTED:
+ * run the observer and ct_fake_quantize separately.  Enqueue-only, no host synchronisation (capturable into a CUDA graph). */
+int ct_dynamic_fake_quantize(const ct_quant_desc* d, int asymmetric, int scale_dtype_arg, const void* x, void* out, void* scale_out,
+                             void* zp_out, int device, void* stream);
+
 /* ---- multi-tensor (whole-model) launches -------------------------------------
  * One persistent launch over `n` independent tensors: the body of the module loop of
  * ModelCompressor.compress_model / decompress_model

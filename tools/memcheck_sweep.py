@@ -199,6 +199,26 @@ def heads_family(dt):
                 ops.fake_quantize_heads(list(pair), [s for s, _ in sz], [z for _, z in sz], a)
 
 
+def dynamic_family(dt):
+    """ct_dynamic_fake_quantize: every strategy it takes (TOKEN up to the widest 32768-column row on the 512-thread CTA, GROUP 16..128
+    on every element rule, TENSOR), ragged row counts that end inside a warp span and a CTA"""
+    schemes = [dict(num_bits=8, type="int", strategy="token"), dict(num_bits=8, type="int", strategy="token", symmetric=False),
+               dict(num_bits=8, type="float", strategy="token"), dict(num_bits=8, type="float", strategy="group", group_size=128),
+               dict(num_bits=8, type="int", strategy="group", group_size=64, symmetric=False),
+               dict(num_bits=4, type="float", strategy="tensor_group", group_size=16, scale_dtype=torch.float8_e4m3fn, zp_dtype=torch.float8_e4m3fn),
+               dict(num_bits=4, type="float", strategy="group", group_size=32, scale_dtype=torch.uint8, zp_dtype=torch.uint8),
+               dict(num_bits=8, type="float", strategy="group", group_size=32, scale_dtype=torch.uint8, zp_dtype=torch.uint8),
+               dict(num_bits=8, type="int", strategy="tensor", symmetric=False)]
+    for shape in ((1, 1, 128), (3, 7, 4104), (2, 5, 1040 * 16), (1, 3, 32768), (1001, 160), (7, 3, 2, 64)):
+        x = torch.randn(shape, device=DEV).to(dt)
+        for kw in schemes:
+            a = qa(dynamic=True, **kw)
+            if kw["strategy"] in ("group", "tensor_group") and shape[-1] % kw["group_size"]:
+                continue
+            gs = torch.full((1,), 64.0, device=DEV) if kw.get("scale_dtype") == torch.float8_e4m3fn else None
+            ops.dynamic_fake_quantize(x, a, global_scale=gs)
+
+
 FAILED = []
 
 
@@ -223,6 +243,8 @@ def main():
                 attempt(observer_family, rows, cols, dt)
         attempt(transform_family, dt)
         attempt(heads_family, dt)
+        if dt != torch.float32:
+            attempt(dynamic_family, dt)
         torch.cuda.synchronize()
         print(f"{dt}: launches so far {N.launch_count()}", flush=True)
     for rows, cols in ((128, 128), (200, 384), (1024, 2048)):
