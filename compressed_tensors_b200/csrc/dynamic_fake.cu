@@ -33,12 +33,6 @@ struct DynParams {
     const float* gs;    // global scale (one float32 on the device) or nullptr
 };
 
-// packed min / max of one 16-byte chunk
-template <class P> __device__ __forceinline__ void chunk_minmax(const uint4& v, uint32_t& mn2, uint32_t& mx2) {
-    mn2 = min2<P>(min2<P>(mn2, v.x), min2<P>(v.y, min2<P>(v.z, v.w)));
-    mx2 = max2<P>(max2<P>(mx2, v.x), max2<P>(v.y, max2<P>(v.z, v.w)));
-}
-
 // ------------------------------------------------------------------------------------
 // TOKEN: one CTA of NT threads per row, up to NT * MAXU chunks of 8 elements
 // ------------------------------------------------------------------------------------
@@ -58,18 +52,18 @@ __global__ void __launch_bounds__(NT) dyn_token_kernel(const uint4* __restrict__
     }
     uint32_t mn2 = v[0].x, mx2 = v[0].x;
 #pragma unroll
-    for (int u = 0; u < MAXU; ++u) chunk_minmax<P>(v[u], mn2, mx2);
+    for (int u = 0; u < MAXU; ++u) obs_chunk_minmax<P>(v[u], mn2, mx2);
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
-        mn2 = min2<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
-        mx2 = max2<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
+        mn2 = min2_nan<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
+        mx2 = max2_nan<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
     }
     if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = mn2; red[1][threadIdx.x >> 5] = mx2; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        for (int w = 1; w < NW; ++w) { mn2 = min2<P>(mn2, red[0][w]); mx2 = max2<P>(mx2, red[1][w]); }
-        const float lo = fminf(fminf(P::lo(mn2), P::hi(mn2)), 0.f);   // min(min_vals, 0)
-        const float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);   // max(max_vals, 0)
+        for (int w = 1; w < NW; ++w) { mn2 = min2_nan<P>(mn2, red[0][w]); mx2 = max2_nan<P>(mx2, red[1][w]); }
+        float lo, hi;
+        obs_range2<P>(mn2, mx2, lo, hi);
         float zq;
         const float s = obs_scale_zp<P::DT>(lo, hi, ASYM, cm.qmin, cm.qmax, zq);
         reinterpret_cast<unsigned short*>(scale_out)[r] = (unsigned short)P::from_float1(s);
@@ -119,18 +113,18 @@ __global__ void __launch_bounds__(256) dyn_group_kernel(const uint4* __restrict_
     for (int k = 0; k < GROUP_UNITS; ++k) {
         const int64_t c = base + k * 32;
         uint32_t mn2 = v[k].x, mx2 = v[k].x;
-        chunk_minmax<P>(v[k], mn2, mx2);
+        obs_chunk_minmax<P>(v[k], mn2, mx2);
 #pragma unroll
         for (int d = 1; d < LPG; d <<= 1) {
-            mn2 = min2<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
-            mx2 = max2<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
+            mn2 = min2_nan<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
+            mx2 = max2_nan<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
         }
         if (c >= n_chunks) continue;
-        const float lo = fminf(fminf(P::lo(mn2), P::hi(mn2)), 0.f);
-        const float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);
+        float lo, hi;
+        obs_range2<P>(mn2, mx2, lo, hi);
         float s, zq = 0.f;
         if (prm.srule == SR_MX) {
-            s = obs_mx_scale<P::DT>(fmaxf(fabsf(lo), fabsf(hi)), prm.cm.bits);
+            s = obs_mx_scale<P::DT>(fmax_nan(fabsf(lo), fabsf(hi)), prm.cm.bits);
         } else if (prm.srule == SR_FP8) {
             uint32_t byte;
             const float st = obs_sym_scale<P::DT>(lo, hi, prm.cm.qmin, prm.cm.qmax);

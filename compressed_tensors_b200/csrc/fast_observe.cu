@@ -30,19 +30,19 @@ struct ObserveQuantPackOp {
         for (int g = 0; g < 4; ++g)
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                mn2 = min2<P>(mn2, w[g][k]);
-                mx2 = max2<P>(mx2, w[g][k]);
+                mn2 = min2_nan<P>(mn2, w[g][k]);
+                mx2 = max2_nan<P>(mx2, w[g][k]);
             }
         if (LPG > 1) {
             const unsigned act = __activemask();   // whole groups are active or inactive together
 #pragma unroll
             for (int d = 1; d < LPG; d <<= 1) {
-                mn2 = min2<P>(mn2, __shfl_xor_sync(act, mn2, d));
-                mx2 = max2<P>(mx2, __shfl_xor_sync(act, mx2, d));
+                mn2 = min2_nan<P>(mn2, __shfl_xor_sync(act, mn2, d));
+                mx2 = max2_nan<P>(mx2, __shfl_xor_sync(act, mx2, d));
             }
         }
-        float lo = fminf(fminf(P::lo(mn2), P::hi(mn2)), 0.f);   // min(min_vals, 0)
-        float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);   // max(max_vals, 0)
+        float lo, hi;
+        obs_range2<P>(mn2, mx2, lo, hi);
 
         // ---- calculate_qparams, each op rounded to T (helpers.py:74-131) ----
         float zq;

@@ -33,21 +33,18 @@ __global__ void __launch_bounds__(256) observe_channel_kernel(const uint4* __res
     }
     uint32_t mn2 = v[0].x, mx2 = v[0].x;
 #pragma unroll
-    for (int u = 0; u < MAXU; ++u) {
-        mn2 = min2<P>(min2<P>(mn2, v[u].x), min2<P>(v[u].y, min2<P>(v[u].z, v[u].w)));
-        mx2 = max2<P>(max2<P>(mx2, v[u].x), max2<P>(v[u].y, max2<P>(v[u].z, v[u].w)));
-    }
+    for (int u = 0; u < MAXU; ++u) obs_chunk_minmax<P>(v[u], mn2, mx2);
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
-        mn2 = min2<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
-        mx2 = max2<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
+        mn2 = min2_nan<P>(mn2, __shfl_xor_sync(0xffffffffu, mn2, d));
+        mx2 = max2_nan<P>(mx2, __shfl_xor_sync(0xffffffffu, mx2, d));
     }
     if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = mn2; red[1][threadIdx.x >> 5] = mx2; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        for (int w = 1; w < 8; ++w) { mn2 = min2<P>(mn2, red[0][w]); mx2 = max2<P>(mx2, red[1][w]); }
-        const float lo = fminf(fminf(P::lo(mn2), P::hi(mn2)), 0.f);   // min(min_vals, 0)
-        const float hi = fmaxf(fmaxf(P::lo(mx2), P::hi(mx2)), 0.f);   // max(max_vals, 0)
+        for (int w = 1; w < 8; ++w) { mn2 = min2_nan<P>(mn2, red[0][w]); mx2 = max2_nan<P>(mx2, red[1][w]); }
+        float lo, hi;
+        obs_range2<P>(mn2, mx2, lo, hi);
         // calculate_qparams, each op rounded to T (helpers.py:74-131)
         float zq;
         const float s = obs_scale_zp<P::DT>(lo, hi, ASYM, cm.qmin, cm.qmax, zq);

@@ -19,6 +19,7 @@
 namespace ctb {
 
 __device__ __forceinline__ uint32_t enc_f32(float f) {          // order-preserving: larger float <=> larger key; every key > 0
+    if (f != f) return 0xffffffffu;                               // a NaN of either sign wins the atomicMax and decodes to NaN
     const uint32_t u = __float_as_uint(f);
     return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
 }
@@ -60,8 +61,8 @@ __global__ void __launch_bounds__(256) minmax_qparams_kernel(const uint4* __rest
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const float a = __uint_as_float(v[u].x), b = __uint_as_float(v[u].y), c = __uint_as_float(v[u].z), d = __uint_as_float(v[u].w);
-                lo = fminf(lo, fminf(fminf(a, b), fminf(c, d)));
-                hi = fmaxf(hi, fmaxf(fmaxf(a, b), fmaxf(c, d)));
+                lo = fmin_nan(lo, fmin_nan(fmin_nan(a, b), fmin_nan(c, d)));
+                hi = fmax_nan(hi, fmax_nan(fmax_nan(a, b), fmax_nan(c, d)));
             }
         }
     } else {
@@ -71,23 +72,19 @@ __global__ void __launch_bounds__(256) minmax_qparams_kernel(const uint4* __rest
 #pragma unroll
             for (int u = 0; u < 4; ++u) v[u] = (i + u * stride < n_vec) ? ldg16_hint(x + i + u * stride, policy) : make_uint4(0, 0, 0, 0);
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                mn2 = min2<P>(min2<P>(mn2, v[u].x), min2<P>(v[u].y, min2<P>(v[u].z, v[u].w)));
-                mx2 = max2<P>(max2<P>(mx2, v[u].x), max2<P>(v[u].y, max2<P>(v[u].z, v[u].w)));
-            }
+            for (int u = 0; u < 4; ++u) obs_chunk_minmax<P>(v[u], mn2, mx2);
         }
-        lo = fminf(P::lo(mn2), P::hi(mn2));
-        hi = fmaxf(P::lo(mx2), P::hi(mx2));
+        obs_range2<P>(mn2, mx2, lo, hi);
     }
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
-        lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, d));
-        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, d));
+        lo = fmin_nan(lo, __shfl_xor_sync(0xffffffffu, lo, d));
+        hi = fmax_nan(hi, __shfl_xor_sync(0xffffffffu, hi, d));
     }
     if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = lo; red[1][threadIdx.x >> 5] = hi; }
     __syncthreads();
     if (threadIdx.x != 0) return;
-    for (int w = 1; w < 8; ++w) { lo = fminf(lo, red[0][w]); hi = fmaxf(hi, red[1][w]); }
+    for (int w = 1; w < 8; ++w) { lo = fmin_nan(lo, red[0][w]); hi = fmax_nan(hi, red[1][w]); }
     atomicMax(slots + 0, enc_f32(-lo));
     atomicMax(slots + 1, enc_f32(hi));
     __threadfence();
@@ -100,7 +97,7 @@ __global__ void __launch_bounds__(256) minmax_qparams_kernel(const uint4* __rest
         // generate_gparam (helpers.py:308-337): 448 * 6 / clamp(max|x|, tiny) in x's dtype, NaN / inf -> 1, as float32.
         // `python_float / tensor` is Tensor.__rtruediv__ = tensor.reciprocal() * python_float: TWO roundings to x's dtype (1 / top, then
         // the product), not one division -- 2688 / 1.745 is 1541 in fp16 this way, 1540 by a correctly rounded quotient.
-        float top = fmaxf(fmaxf(fabsf(lo), fabsf(hi)), obs_tiny<P::DT>());
+        float top = fmax_nan(fmax_nan(fabsf(lo), fabsf(hi)), obs_tiny<P::DT>());
         float g = obs_round<P::DT>(__fmul_rn(obs_round<P::DT>(__frcp_rn(top)), 2688.0f));
         if (g != g || fabsf(g) == __int_as_float(0x7f800000)) g = 1.0f;
         *reinterpret_cast<float*>(scale_out) = g;

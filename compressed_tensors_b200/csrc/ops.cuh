@@ -70,12 +70,13 @@ template <class P, int ZP> __device__ __forceinline__ uint32_t zp_t2(const RawQP
     }
 }
 
-// fp32 compute dtype: clamped, un-rounded value
-template <int ZP>
+// fp32 compute dtype: clamped, un-rounded value (NAN_CLAMP as in clamp2)
+template <int ZP, bool NAN_CLAMP = false>
 __device__ __forceinline__ float scaled_clamped_f32(float x, float s, uint32_t zpbits, const Common& cm) {
     float t = __fdiv_rn(x, s);
     if (ZP) t = __fadd_rn(t, __uint_as_float(zpbits));
-    return fminf(fmaxf(t, cm.qmin), cm.qmax);
+    if constexpr (NAN_CLAMP) return fmin_nan(fmax_nan(t, cm.qmin), cm.qmax);
+    else return fminf(fmaxf(t, cm.qmin), cm.qmax);
 }
 
 // rounded (integer-valued, sign of zero preserved) pair in T
@@ -400,6 +401,7 @@ struct UnpackDequantOp {
 
 // ------------------------------------------------------------------------------------
 // FakeQuant: x (8 x T) -> quantize -> dequantize -> 8 x T   (forward_helpers.py:180-215)
+//   a NaN input or scale gives NaN, as in the reference: the clamp propagates it
 // ------------------------------------------------------------------------------------
 template <class P, int KIND, int ZP>
 struct FakeQuantOp {
@@ -414,7 +416,7 @@ struct FakeQuantOp {
         if constexpr (P::DT == CT_F32) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                float t = scaled_clamped_f32<ZP>(__uint_as_float(w[k]), sc.s, zp2, cm);
+                float t = scaled_clamped_f32<ZP, true>(__uint_as_float(w[k]), sc.s, zp2, cm);
                 if constexpr (KIND == QF8) t = e4m3_to_f32(f32_to_e4m3_byte(t));
                 else t = rintf(t);
                 o[k] = __float_as_uint(dq_tail_f32<ZP>(t, zp2, s2));
@@ -422,7 +424,7 @@ struct FakeQuantOp {
         } else {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                uint32_t t = scaled_clamped2<P, ZP != 0, SLOW>(w[k], sc, zp2, cm.qmin2, cm.qmax2);
+                uint32_t t = scaled_clamped2<P, ZP != 0, SLOW, true>(w[k], sc, zp2, cm.qmin2, cm.qmax2);
                 if constexpr (KIND == QF8) t = round_fp8_2<P>(t);
                 else t = round_int2<P, KIND == QI_WIDE>(t);
                 o[k] = dq_tail2<P, ZP>(t, zp2, s2);

@@ -80,6 +80,16 @@ template <class P> __device__ __forceinline__ uint32_t min2(uint32_t a, uint32_t
     typename P::T2 r = __hmin2(*reinterpret_cast<typename P::T2*>(&a), *reinterpret_cast<typename P::T2*>(&b));
     return *reinterpret_cast<uint32_t*>(&r);
 }
+// NaN-propagating packed min / max (max.NaN / min.NaN): torch.clamp, amin and amax give NaN where an operand is NaN, while
+// max2 / min2 return the other operand
+template <class P> __device__ __forceinline__ uint32_t max2_nan(uint32_t a, uint32_t b) {
+    typename P::T2 r = __hmax2_nan(*reinterpret_cast<typename P::T2*>(&a), *reinterpret_cast<typename P::T2*>(&b));
+    return *reinterpret_cast<uint32_t*>(&r);
+}
+template <class P> __device__ __forceinline__ uint32_t min2_nan(uint32_t a, uint32_t b) {
+    typename P::T2 r = __hmin2_nan(*reinterpret_cast<typename P::T2*>(&a), *reinterpret_cast<typename P::T2*>(&b));
+    return *reinterpret_cast<uint32_t*>(&r);
+}
 template <class P> __device__ __forceinline__ uint32_t dup2(float v) {
     uint32_t h = P::from_float1(v);
     return h | (h << 16);
@@ -123,23 +133,29 @@ __device__ __forceinline__ float quot(float x, const ScaleCtx& c) {
 
 // x pair (raw T2 bits) -> clamped value in T, before rounding to the quantized grid.
 // zp2: zero point already converted to T (zero_point.to(x.dtype)), duplicated in both halves.
+// NAN_CLAMP keeps a NaN through the clamp as torch.clamp does (fake_quantize, whose output is a float); the ops that produce codes
+// leave it off, since the code of a NaN is undefined in the reference.
+template <class P, bool NAN_CLAMP>
+__device__ __forceinline__ uint32_t clamp2(uint32_t t, uint32_t qmin2, uint32_t qmax2) {
+    if constexpr (NAN_CLAMP) return min2_nan<P>(max2_nan<P>(t, qmin2), qmax2);
+    else return min2<P>(max2<P>(t, qmin2), qmax2);
+}
 // out-of-line IEEE-division variant (rare: scale outside [2^-100, 2^100]); scalar by-value
 // arguments so that nothing is forced into local memory
-template <class P, bool HAS_ZP>
+template <class P, bool HAS_ZP, bool NAN_CLAMP>
 __device__ __noinline__ uint32_t scaled_clamped2_slow(uint32_t xv, float s, uint32_t zp2, uint32_t qmin2, uint32_t qmax2) {
     uint32_t t = P::pack(__fdiv_rn(P::lo(xv), s), __fdiv_rn(P::hi(xv), s));
     if (HAS_ZP) t = add2<P>(t, zp2);
-    return min2<P>(max2<P>(t, qmin2), qmax2);
+    return clamp2<P, NAN_CLAMP>(t, qmin2, qmax2);
 }
-template <class P, bool HAS_ZP, bool SLOW>
+template <class P, bool HAS_ZP, bool SLOW, bool NAN_CLAMP = false>
 __device__ __forceinline__ uint32_t scaled_clamped2(uint32_t xv, const ScaleCtx& c, uint32_t zp2, uint32_t qmin2, uint32_t qmax2) {
-    if constexpr (SLOW) return scaled_clamped2_slow<P, HAS_ZP>(xv, c.s, zp2, qmin2, qmax2);
+    if constexpr (SLOW) return scaled_clamped2_slow<P, HAS_ZP, NAN_CLAMP>(xv, c.s, zp2, qmin2, qmax2);
     float q0 = quot<P, false>(P::lo(xv), c);
     float q1 = quot<P, false>(P::hi(xv), c);
     uint32_t t = P::pack(q0, q1);                // scaled = x / scale          (rounds to T)
     if (HAS_ZP) t = add2<P>(t, zp2);             // scaled += zero_point.to(T)  (rounds to T)
-    t = min2<P>(max2<P>(t, qmin2), qmax2);       // torch.clamp
-    return t;
+    return clamp2<P, NAN_CLAMP>(t, qmin2, qmax2);   // torch.clamp
 }
 
 // round-half-even of a clamped T2 pair; result n has two's complement in the low bits of each half
@@ -280,6 +296,25 @@ CT_HD float load_as_f32(const void* p, int64_t i, int dt) {
     }
     default: return 0.f;
     }
+}
+// NaN-propagating min / max (min.NaN / max.NaN on the device), the scalar counterparts of min2_nan / max2_nan
+CT_HD float fmin_nan(float a, float b) {
+#ifdef __CUDA_ARCH__
+    float r;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+#else
+    return (a != a || b != b) ? a + b : fminf(a, b);
+#endif
+}
+CT_HD float fmax_nan(float a, float b) {
+#ifdef __CUDA_ARCH__
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+#else
+    return (a != a || b != b) ? a + b : fmaxf(a, b);
+#endif
 }
 CT_HD float clamp_nan(float v, float lo, float hi) {
     // torch.clamp propagates NaN

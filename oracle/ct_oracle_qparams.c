@@ -29,11 +29,12 @@ int orc_calculate_qparams(const void* mn, const void* mx, int dt, void* scale_ou
     const float range = qmax - qmin;      /* 0-dim fp32 tensor arithmetic in the reference */
     for (int64_t i = 0; i < n; ++i) {
         float lo = load_as_f32(mn, i, dt), hi = load_as_f32(mx, i, dt);
-        lo = lo < 0.0f ? lo : 0.0f;       /* torch.min(x, 0): for -0.0 vs 0.0 either is fine downstream */
-        hi = hi > 0.0f ? hi : 0.0f;
+        /* torch.min(x, 0) / torch.max(x, 0) keep a NaN; for -0.0 vs 0.0 either is fine downstream */
+        lo = (lo != lo || lo < 0.0f) ? lo : 0.0f;
+        hi = (hi != hi || hi > 0.0f) ? hi : 0.0f;
         float s, z;
         if (symmetric) {
-            const float m = fabsf(lo) > fabsf(hi) ? fabsf(lo) : fabsf(hi);
+            const float m = (lo != lo || fabsf(lo) > fabsf(hi)) ? fabsf(lo) : fabsf(hi);   /* torch.max propagates NaN */
             s = rnd(m / (range / 2.0f), dt);
             z = 0.0f;
         } else {

@@ -2,6 +2,7 @@
     compute-sanitizer --tool memcheck --error-exitcode 9 python tools/memcheck_sweep.py
 so that out-of-bounds / misaligned accesses of the generic kernels' tails and of the TMA ring's last tiles show up.  Results are
 not checked here (the -m gpu tests do that against the oracle); the script only has to touch every code path once."""
+import itertools
 import os
 import sys
 
@@ -209,8 +210,12 @@ def dynamic_family(dt):
                dict(num_bits=4, type="float", strategy="group", group_size=32, scale_dtype=torch.uint8, zp_dtype=torch.uint8),
                dict(num_bits=8, type="float", strategy="group", group_size=32, scale_dtype=torch.uint8, zp_dtype=torch.uint8),
                dict(num_bits=8, type="int", strategy="tensor", symmetric=False)]
-    for shape in ((1, 1, 128), (3, 7, 4104), (2, 5, 1040 * 16), (1, 3, 32768), (1001, 160), (7, 3, 2, 64)):
+    for shape, planted in itertools.product(((1, 1, 128), (3, 7, 4104), (2, 5, 1040 * 16), (1, 3, 32768), (1001, 160), (7, 3, 2, 64)),
+                                            (False, True)):
         x = torch.randn(shape, device=DEV).to(dt)
+        if planted:   # NaN and +-inf take the NaN-propagating reductions and clamps
+            flat = x.view(-1)
+            flat[::97], flat[5::131], flat[7::151] = float("nan"), float("inf"), float("-inf")
         for kw in schemes:
             a = qa(dynamic=True, **kw)
             if kw["strategy"] in ("group", "tensor_group") and shape[-1] % kw["group_size"]:
