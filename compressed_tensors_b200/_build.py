@@ -41,6 +41,7 @@ SOURCES = [
     "cpu_twin.cu",
     "fast_observe.cu",
     "dynamic_fake.cu",
+    "observe_block_mx.cu",
 ]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + ["../../include/ct_b200.h"]   # every header: a stale object is a silent wrong build
 

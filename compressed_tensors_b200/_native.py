@@ -40,7 +40,7 @@ DT = {
 # ct_batch_op_t
 (OP_QUANTIZE_PACK, OP_UNPACK_DEQUANTIZE, OP_QUANTIZE, OP_DEQUANTIZE, OP_FAKE_QUANTIZE, OP_PACK_INT32, OP_UNPACK_INT32,
  OP_OBSERVE_QUANTIZE_PACK, OP_QUANTIZE_PACK_FP4, OP_UNPACK_DEQUANTIZE_FP4, OP_OBSERVE_QUANTIZE_PACK_FP4,
- OP_SPARSE24_QUANTIZE_PACK, OP_SPARSE24_UNPACK_DEQUANTIZE) = range(13)
+ OP_SPARSE24_QUANTIZE_PACK, OP_SPARSE24_UNPACK_DEQUANTIZE, OP_OBSERVE_QUANTIZE_BLOCK, OP_OBSERVE_QUANTIZE_MX) = range(15)
 
 Q_INT, Q_FLOAT, Q_FP4 = 0, 1, 2
 DT_E8M0 = 8  # uint8 MX scale exponent as stored (CT_E8M0)
@@ -143,6 +143,8 @@ _PROTOS = {
     "ct_awq_repack_int4": (_int, [_vp, _vp, _i64, _i64, _int, _vp]),
     "ct_awq_repack_zeros_int4": (_int, [_vp, _vp, _i64, _i64, _int, _vp]),
     "ct_observe_quantize_channel": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),
+    "ct_observe_quantize_block": (_int, [_descp, _vp, _vp, _vp, _int, _vp]),
+    "ct_observe_quantize_mx": (_int, [_descp, _vp, _vp, _vp, _int, _vp]),
     "ct_observe_tensor": (_int, [_descp, _vp, _int, _vp, _vp, _int, _vp]),
     "ct_observe_quantize_tensor": (_int, [_descp, _vp, _vp, _vp, _vp, _int, _vp]),
     "ct_dynamic_fake_quantize": (_int, [_descp, _int, _int, _vp, _vp, _vp, _vp, _int, _vp]),

@@ -408,6 +408,7 @@ static int check_dtypes(int op, const ct_quant_desc& d, bool has_zp) {
 
 int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in, const void* const* scale,
                 const void* const* zp, const int32_t* const* g_idx, void* const* out, int device, cudaStream_t stream) {
+    if (op == CT_OP_OBSERVE_QUANTIZE_BLOCK || op == CT_OP_OBSERVE_QUANTIZE_MX) return run_observe_block_mx(op, n, descs, in, scale, out, device, stream);
     const bool bits_op = (op == CT_OP_PACK_INT32 || op == CT_OP_UNPACK_INT32);
     if (n < 0 || (n > 0 && (!descs || !in || (!scale && !bits_op) || !out))) { set_error("null table"); return CT_E_ARG; }
     if (device == CT_DEVICE_CPU) {

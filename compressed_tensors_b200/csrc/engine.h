@@ -66,6 +66,9 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
                 const void* const* zp, const int32_t* const* g_idx, void* const* out, int device, cudaStream_t stream);
 
 int check_device(int device);
+// the fused BLOCK / MX observers (observe_block_mx.cu): ct_batched ops CT_OP_OBSERVE_QUANTIZE_BLOCK / _MX; scale[i] are OUTPUTS
+int run_observe_block_mx(int op, int n, const ct_quant_desc* descs, const void* const* in, const void* const* scale, void* const* out,
+                         int device, cudaStream_t stream);
 Common make_common(int p_dt, int qtype, int bits);   // clamp bounds of a (qtype, bits) in the compute dtype p_dt (dispatch.cu)
 
 // ---- CPU twins (cpu_twin.cu): host code behind device = CT_DEVICE_CPU, same per-element source as the generic kernels ----

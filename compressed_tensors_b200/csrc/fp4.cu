@@ -4,6 +4,7 @@
 // Reference: quantization/utils/fp4_utils.py:77-98, compressors/nvfp4/helpers.py:108-193,
 // compressors/nvfp4/base.py:73-128, compressors/mx_utils.py:18-44.
 #include "generic.cuh"
+#include "observe_core.cuh"
 
 namespace ctb {
 
@@ -46,18 +47,10 @@ __global__ void __launch_bounds__(256) fp4_unpackdeq_generic_kernel(const __grid
     }
 }
 
-// 127 + floor(log2(scale)) with log2 and floor in the scale's dtype, -> int32 -> uint8 (wraps); mx_utils.py:30-31
+// 127 + floor(log2(scale)) with log2 and floor in the scale's dtype, -> int32 -> uint8 (wraps); mx_utils.py:30-31 (observe_core.cuh)
 __global__ void __launch_bounds__(256) mx_scale_compress_kernel(const void* __restrict__ s, int dt, uint8_t* __restrict__ out, int64_t n) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float v = load_as_f32(s, i, dt);
-        // exact for powers of two (what the reference's MX observer produces); log2f elsewhere
-        float l;
-        const uint32_t u = __float_as_uint(v);
-        if (v > 0.f && (u & 0x007fffffu) == 0u && (u >> 23) != 0u && (u >> 23) != 255u) l = (float)((int)(u >> 23) - 127);
-        else l = floorf(rnd_dt(log2f(v), dt));
-        const int e = (l != l || isinf(l)) ? (int)0x80000000 : (int)l;
-        out[i] = (uint8_t)(uint32_t)(127 + (long long)e);
-    }
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        out[i] = (uint8_t)mx_scale_code(load_as_f32(s, i, dt), dt);
 }
 
 // 2.0 ** (e - 127).to(bfloat16) -> bfloat16; mx_utils.py:43-44

@@ -88,4 +88,17 @@ template <int DT> CT_HD float obs_mx_scale(float amax, int num_bits) {
     return s == 0.f ? 1.0f : s;
 }
 
+// compress_mx_scale (compressors/mx_utils.py:18-31) of one scale v held in dtype dt: 127 + floor(log2(v)) with log2 and floor in dt,
+// .to(int32), .to(uint8) (wraps).  Exact for powers of two (what obs_mx_scale produces); log2f elsewhere.  inf / NaN / 0 take int32's
+// minimum, as torch's conversion gives on x86, so they store 127.
+CT_HD uint32_t mx_scale_code(float v, int dt) {
+    float l;
+    uint32_t u;
+    memcpy(&u, &v, 4);
+    if (v > 0.f && (u & 0x007fffffu) == 0u && (u >> 23) != 0u && (u >> 23) != 255u) l = (float)((int)(u >> 23) - 127);
+    else l = floorf(rnd_dt(log2f(v), dt));
+    const int e = (l != l || isinf(l)) ? (int)0x80000000 : (int)l;
+    return (uint32_t)(uint8_t)(uint32_t)(127 + (long long)e);
+}
+
 }  // namespace ctb

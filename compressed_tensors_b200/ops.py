@@ -58,6 +58,7 @@ __all__ = [
     "observe_quantize",
     "observe_quantize_pack",
     "observe_quantize_pack_nvfp4",
+    "observe_quantize_mx",
     "observe_tensor_qparams",
     "observe_tensor_gparam",
     "dequantize_block_fp8",
@@ -1079,6 +1080,113 @@ def observe_quantize_pack_nvfp4(x: torch.Tensor, args, global_scale: Optional[to
     return _back(packed, x), _back(scale.to(torch.float8_e4m3fn), x), _back(gs, x)
 
 
+def _block_desc(rows: int, cols: int, bh: int, bw: int, x_dtype: torch.dtype) -> N.QuantDesc:
+    """descriptor of `ct_observe_quantize_block` / batched op OP_OBSERVE_QUANTIZE_BLOCK for an fp8 weight [rows, cols] in blocks [bh, bw]"""
+    d = N.QuantDesc()
+    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, bh, bw, -(-cols // bw)
+    d.x_dtype = d.scale_dtype = d.compute_dtype = N.DT[x_dtype]
+    d.zp_dtype, d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT_NONE, N.DT[torch.float8_e4m3fn], N.DT_NONE, N.Q_FLOAT, 8
+    d.global_scale, d.seff_dtype, d.aux = None, N.DT_NONE, None
+    return d
+
+
+def _mx_desc(rows: int, cols: int, bits: int, x_dtype: torch.dtype) -> N.QuantDesc:
+    """descriptor of `ct_observe_quantize_mx` / batched op OP_OBSERVE_QUANTIZE_MX: MXFP4 (bits 4) or MXFP8 (bits 8), groups of 32"""
+    d = N.QuantDesc()
+    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, 1, 32, cols // 32
+    d.x_dtype = d.compute_dtype = N.DT[x_dtype]
+    d.scale_dtype, d.zp_dtype, d.out_dtype = N.DT_E8M0, N.DT_NONE, N.DT_NONE
+    d.qtype, d.num_bits = (N.Q_FP4, 4) if bits == 4 else (N.Q_FLOAT, 8)
+    d.q_dtype = N.DT[torch.uint8] if bits == 4 else N.DT[torch.float8_e4m3fn]
+    d.global_scale, d.seff_dtype, d.aux = None, N.DT_NONE, None
+    return d
+
+
+def _aligned(*tensors: torch.Tensor) -> bool:
+    return all(t.data_ptr() % 16 == 0 for t in tensors)
+
+
+def _observe_quantize_block(x: torch.Tensor, args, qtype: int, bits: int, symmetric: bool):
+    """observe_quantize for the BLOCK strategy: the fused kernel for symmetric fp8 codes of bf16 / fp16 weights whose rows and block
+    width are a multiple of 8 elements; otherwise torch block min / max -> calculate_qparams -> quantize, with identical results"""
+    from .quantization.utils.helpers import calculate_qparams
+
+    bs = getattr(args, "block_structure", None)
+    if bs is None or len(bs) != 2:
+        raise ValueError("block quantization needs a block_structure [rows, cols]")
+    bh, bw = int(bs[0]), int(bs[1])
+    rows, cols = x.shape
+    nrb, ncb = -(-rows // bh), -(-cols // bw)
+    qdt = torch.float8_e4m3fn if qtype == N.Q_FLOAT else torch.int8
+    if x.device.type == "meta":
+        zp = None if symmetric else torch.empty((nrb, ncb), dtype=qdt if qtype == N.Q_FLOAT else torch.int8, device="meta")
+        return (torch.empty((rows, cols), dtype=qdt, device="meta"), torch.empty((nrb, ncb), dtype=x.dtype, device="meta"), zp)
+    idx = _dev_index(x)
+    xd = _to_dev(x, idx).contiguous()
+    if (idx != _CPU and qtype == N.Q_FLOAT and bits == 8 and symmetric and x.dtype in (torch.bfloat16, torch.float16)
+            and cols % 8 == 0 and bw % 8 == 0 and rows * cols > 0 and _aligned(xd)):
+        scale = torch.empty((nrb, ncb), dtype=x.dtype, device=xd.device)
+        out = torch.empty((rows, cols), dtype=qdt, device=xd.device)
+        d = _block_desc(rows, cols, bh, bw, x.dtype)
+        rc = N.lib().ct_observe_quantize_block(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(out), idx, N.stream_ptr(idx))
+        N.check(rc, "observe_quantize")
+        return _back(out, x), _back(scale, x), None
+    # unfused: min / max per block over the elements that exist (zero padding is neutral: the rule clamps min <= 0 <= max)
+    xp = torch.nn.functional.pad(xd, (0, ncb * bw - cols, 0, nrb * bh - rows)).reshape(nrb, bh, ncb, bw)
+    scale, zp = calculate_qparams(xp.amin(dim=(1, 3)), xp.amax(dim=(1, 3)), args)
+    zp = None if symmetric else zp
+    out = quantize(xd, scale, zp, args, dtype=qdt)
+    return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+
+
+def _is_mx(args) -> bool:
+    return (_type_name(args) == "float" and int(getattr(args, "num_bits", 0)) in (4, 8) and _strategy_name(args) == "group"
+            and int(getattr(args, "group_size", 0) or 0) == 32 and getattr(args, "scale_dtype", None) == torch.uint8)
+
+
+@torch.no_grad()
+def observe_quantize_mx(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Tensor]:
+    """MXFP4 / MXFP8 "calibrate + compress" of one weight x [R, C] (bf16 / fp16): returns the compressor's tensors
+        MXFP4: (weight_packed uint8 [R, C/2], weight_scale uint8 [R, C/32])
+        MXFP8: (weight float8_e4m3fn [R, C],   weight_scale uint8 [R, C/32])
+    -- what the reference produces with
+        scale, _ = calculate_qparams(group min, group max, args)     (utils/helpers.py:50-137: generate_mx_scales and
+                                                                      maybe_convert_from_mx_exp, quantization/utils/mxfp_utils.py)
+        MXFP4PackedCompressor.compress / MXFP8QuantizationCompressor.compress({"weight", "weight_scale"})
+                                                                     (quantize, pack_fp4_to_uint8 for MXFP4, compress_mx_scale)
+    bit for bit, in ONE pass over the weight (`ct_observe_quantize_mx`): max |x| per group of 32, the power-of-two scale, its E8M0
+    exponent and the codes come out of registers.  Weights the kernel does not take (fp32, C % 32 != 0, no CUDA device) run the same
+    steps unfused: torch min / max per group, calculate_qparams, quantize(_pack_fp4), compress_mx_scale."""
+    from .quantization.utils.helpers import calculate_qparams
+
+    if not _is_mx(args):
+        raise ValueError("observe_quantize_mx needs MX args (float, 4 or 8 bits, group, group_size 32, scale_dtype uint8)")
+    if not bool(getattr(args, "symmetric", True)):
+        raise NotImplementedError("MX formats are symmetric")
+    if x.ndim != 2:
+        raise ValueError("observe_quantize_mx expects a 2-D weight")
+    bits = int(args.num_bits)
+    rows, cols = x.shape
+    if cols % 32 != 0:
+        raise ValueError(f"tensor column shape must be divisble by the given group_size 32 but got {cols}")
+    q_shape, q_dt = ((rows, cols // 2), torch.uint8) if bits == 4 else ((rows, cols), torch.float8_e4m3fn)
+    if x.device.type == "meta":
+        return torch.empty(q_shape, dtype=q_dt, device="meta"), torch.empty((rows, cols // 32), dtype=torch.uint8, device="meta")
+    idx = _dev_index(x)
+    xd = _to_dev(x, idx).contiguous()
+    if idx != _CPU and x.dtype in (torch.bfloat16, torch.float16) and rows * cols > 0 and _aligned(xd):
+        scale = torch.empty((rows, cols // 32), dtype=torch.uint8, device=xd.device)
+        out = torch.empty(q_shape, dtype=q_dt, device=xd.device)
+        d = _mx_desc(rows, cols, bits, x.dtype)
+        rc = N.lib().ct_observe_quantize_mx(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(out), idx, N.stream_ptr(idx))
+        N.check(rc, "observe_quantize_mx")
+        return _back(out, x), _back(scale, x)
+    g = xd.unflatten(-1, (-1, 32))
+    scale, _ = calculate_qparams(g.amin(-1), g.amax(-1), args)
+    out = quantize_pack_fp4(xd, scale, None, args) if bits == 4 else quantize(xd, scale, None, args, dtype=torch.float8_e4m3fn)
+    return _back(out, x), _back(compress_mx_scale(scale, torch.uint8), x)
+
+
 @torch.no_grad()
 def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
     """Memoryless min-max observer + quantize (+ pack_to_int32 when `pack`) in ONE pass over the weight, for the strategies with a
@@ -1090,6 +1198,8 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
       TENSOR (one scale)         : `ct_observe_quantize_tensor` -- grid-wide min / max, calculate_qparams by the last CTA, then the
                                    streaming quantize kernel with the device-resident scale; no host round trip (the FP8 preset)
       GROUP + pack               : `observe_quantize_pack`
+      BLOCK (FP8_BLOCK)          : `ct_observe_quantize_block` -- one CTA per block: min / max, calculate_qparams, fp8 codes; returns
+                                   (float8_e4m3fn [R, C], scale in x.dtype [ceil(R / bh), ceil(C / bw)], None)
     Everything else runs the observer with torch reductions on the device and then the quantize kernel."""
     from .quantization.utils.helpers import calculate_qparams
 
@@ -1102,6 +1212,8 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
         raise ValueError("pack-quantized compression needs integer quantization")
     if strategy == "group" and pack:
         return observe_quantize_pack(x, args)
+    if strategy == "block" and not pack:
+        return _observe_quantize_block(x, args, qtype, bits, symmetric)
     rows, cols = x.shape
     idx = _dev_index(x)
     xd = _to_dev(x, idx).contiguous()
@@ -1192,6 +1304,10 @@ def _validate_problem(op: int, i: int, prob, on_cuda: Optional[int]) -> None:
         want = (n, _DT_SIZE.get(d.x_dtype), n // 2, 1)
     elif op == N.OP_UNPACK_DEQUANTIZE_FP4:
         want = (n // 2, 1, n, _DT_SIZE.get(d.out_dtype))
+    elif op == N.OP_OBSERVE_QUANTIZE_BLOCK:
+        want = (n, _DT_SIZE.get(d.x_dtype), n, 1)
+    elif op == N.OP_OBSERVE_QUANTIZE_MX:
+        want = (n, _DT_SIZE.get(d.x_dtype), n // 2 if d.qtype == N.Q_FP4 else n, 1)
     elif op == N.OP_SPARSE24_QUANTIZE_PACK:          # kept codes [rows, cols/2] as a 4-bit stream; the bitmask (d.aux) is the caller's business
         want = (n, _DT_SIZE.get(d.x_dtype), rows * (-(-(cols // 2) * bits // 32)), 4)
     elif op == N.OP_SPARSE24_UNPACK_DEQUANTIZE:

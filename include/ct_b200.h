@@ -255,6 +255,25 @@ int ct_observe_quantize_channel(const ct_quant_desc* d, const void* x, void* sca
 int ct_observe_tensor(const ct_quant_desc* d, const void* x, int kind, void* scale_out, void* zp_out, int device, void* stream);
 int ct_observe_quantize_tensor(const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, void* q_out, int device, void* stream);
 
+/* ---- one-pass observe + compress for the BLOCK and MX weight formats ------------------------------------------
+ * The memoryless min-max observer and calculate_qparams (quantization/utils/helpers.py:50-137) fused with the compressor body, so the
+ * weight x [rows, cols] (bf16 / fp16, contiguous, cols % 8 == 0, x and q_out 16-byte aligned) is read once.
+ * ct_observe_quantize_block: FP8_BLOCK.  d: rdiv = block rows, cdiv = block columns (cdiv % 8 == 0), s_row_stride = ceil(cols / cdiv),
+ *   qtype CT_Q_FLOAT, q_dtype CT_F8E4M3, scale_dtype = compute_dtype = x_dtype, zp_dtype CT_NONE.  Per block (edge blocks of a ragged shape
+ *   over the elements that exist): max(|min|, |max|) / 448 in x's dtype (0 -> eps), then quantize (forward_helpers.py:523-546) with it.
+ *     scale_out  x dtype [ceil(rows / rdiv), ceil(cols / cdiv)];  q_out  float8_e4m3fn [rows, cols]
+ * ct_observe_quantize_mx: MXFP4 / MXFP8.  d: rdiv = 1, cdiv = 32, s_row_stride = cols / 32 (cols % 32 == 0), scale_dtype CT_E8M0,
+ *   compute_dtype = x_dtype, zp_dtype CT_NONE; qtype CT_Q_FP4 (num_bits 4) or CT_Q_FLOAT (num_bits 8, q_dtype CT_F8E4M3).  Per group:
+ *   generate_mx_scales / maybe_convert_from_mx_exp of max |x| (quantization/utils/mxfp_utils.py:47-139), quantize, and the layouts of
+ *   MXFP4PackedCompressor / MXFP8QuantizationCompressor.compress (compressors/mxfp4/base.py, compressors/mxfp8/base.py):
+ *     scale_out  uint8 [rows, cols / 32] (compress_mx_scale, compressors/mx_utils.py:18-31)
+ *     q_out      uint8 [rows, cols / 2] (E2M1, element 2j in the low nibble) or float8_e4m3fn [rows, cols]
+ * A NaN in a block gives a NaN block scale (and NaN-derived codes).  Anything else -- fp32 x, cols % 8 != 0, a zero point or a global
+ * scale, device = CT_DEVICE_CPU -- returns CT_E_UNSUPPORTED: run the observer and ct_quantize / ct_quantize_pack_fp4 separately.
+ * Enqueue-only.  ct_batched ops CT_OP_OBSERVE_QUANTIZE_BLOCK / _MX run many weights in one launch. */
+int ct_observe_quantize_block(const ct_quant_desc* d, const void* x, void* scale_out, void* q_out, int device, void* stream);
+int ct_observe_quantize_mx(const ct_quant_desc* d, const void* x, void* scale_out_e8m0, void* q_out, int device, void* stream);
+
 /* ---- dynamic activation quantization in one pass ---------------------------------------------------
  * replaces compute_dynamic_scales_and_zp (quantization/utils/helpers.py:140-195) followed by fake_quantize (forward.py:148-181), the
  * dynamic branch of forward_quantize (forward.py:292-329): the memoryless min-max observer and calculate_qparams (helpers.py:50-137)
@@ -296,7 +315,9 @@ typedef enum ct_batch_op_t {
     CT_OP_UNPACK_DEQUANTIZE_FP4 = 9, /* in nibbles -> out float (ct_unpack_dequantize_fp4) */
     CT_OP_OBSERVE_QUANTIZE_PACK_FP4 = 10, /* in x -> out nibbles; scale[i] (float8_e4m3fn) is an OUTPUT (ct_observe_quantize_pack_nvfp4) */
     CT_OP_SPARSE24_QUANTIZE_PACK = 11,    /* in x       -> out packed int32 [rows, cols/16] + descs[i].aux = bitmask OUT (ct_sparse24_quantize_pack_int4) */
-    CT_OP_SPARSE24_UNPACK_DEQUANTIZE = 12 /* in packed  -> out float; descs[i].aux = bitmask IN (ct_sparse24_unpack_dequantize_int4) */
+    CT_OP_SPARSE24_UNPACK_DEQUANTIZE = 12, /* in packed  -> out float; descs[i].aux = bitmask IN (ct_sparse24_unpack_dequantize_int4) */
+    CT_OP_OBSERVE_QUANTIZE_BLOCK = 13,     /* in x -> out fp8 codes; scale[i] (x dtype, one per block) is an OUTPUT (ct_observe_quantize_block) */
+    CT_OP_OBSERVE_QUANTIZE_MX = 14         /* in x -> out nibbles / fp8 codes; scale[i] (E8M0 uint8) is an OUTPUT (ct_observe_quantize_mx) */
 } ct_batch_op_t;
 int ct_batched(int op, int n, const ct_quant_desc* descs, const void* const* in, const void* const* scale,
                const void* const* zp, void* const* out, int device, void* stream);
