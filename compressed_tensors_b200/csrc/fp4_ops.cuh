@@ -74,7 +74,7 @@ __device__ __forceinline__ float fp4_zp_value(uint32_t byte) {
 // Division: q = RN(x / s) through the correctly rounded reciprocal r = RN(1/s) and one residual step
 //   q0 = x r,  e = fma(-q0, s, x),  q1 = fma(e, r, q0)
 // (exhaustively checked against div.rn for every 16-bit x and every scale significand by ct_selftest_fp4_division);
-// groups whose effective scale falls outside [2^-100, 2^10] take div.rn per element.
+// groups whose effective scale falls outside [2^-100, 2^10] (negative ones included) take div.rn per element.
 // ------------------------------------------------------------------------------------
 // per-tile constants of the ops that divide a scale by the tensor's global scale
 struct Fp4DqTile {
@@ -133,13 +133,13 @@ struct Fp4NvQuantPackOp {
             const uint32_t xc = CLAMP ? clamp_x(w[j]) : w[j];
             t[2 * j] = quotient(P::lo(xc), s, rcp);
             t[2 * j + 1] = quotient(P::hi(xc), s, rcp);
-            // the reference's in-place add of the zero point.  Without one nothing is added: the residual step already turns
-            // x = -0.0 into +0.0 (fma(+0, r, -0) = +0) and, with |s| <= 2^10, no non-zero 16-bit x underflows to -0.0
+            // the reference's in-place add of the zero point.  Without one nothing is added: with s in (0, 2^10] the residual step
+            // already turns x = -0.0 into +0.0 (fma(+0, r, -0) = +0) and no non-zero 16-bit x underflows to -0.0
             if constexpr (ZK != FZ_NONE) { t[2 * j] = __fadd_rn(t[2 * j], z); t[2 * j + 1] = __fadd_rn(t[2 * j + 1], z); }
         }
         return f32x8_to_e2m1x8(t[0], t[1], t[2], t[3], t[4], t[5], t[6], t[7]);
     }
-    // out of line, everything by value: a unit whose effective scale is outside [2^-100, 2^10] (or 0 / inf / NaN) -> IEEE division
+    // out of line, everything by value: a unit whose effective scale is outside [2^-100, 2^10] (or <= 0 / inf / NaN) -> IEEE division
     // per element.  One call per unit so that the caller's registers never have to be spilled to be indexed.
     __device__ static __noinline__ uint4 unit_slow(uint4 c0, uint4 c1, uint4 c2, uint4 c3, float s0, float s1, float z0, float z1, int off) {
         const uint4 c[4] = {c0, c1, c2, c3};
@@ -152,8 +152,10 @@ struct Fp4NvQuantPackOp {
             uint32_t word = 0;
 #pragma unroll 1
             for (int j = 0; j < 4; ++j) {
-                const float t0 = __fadd_rn(__fdiv_rn(P::lo(w[j]), s), z);
-                const float t1 = __fadd_rn(__fdiv_rn(P::hi(w[j]), s), z);
+                // the trailing + 0.0f maps a zero quotient to +0.0 as the reference's torch.sign does: x / s is -0.0 for x = -0.0
+                // under s > 0 and for x = +0.0 under s < 0, and a -0.0 zero point (fp8 byte 0x80) keeps it so
+                const float t0 = __fadd_rn(__fadd_rn(__fdiv_rn(P::lo(w[j]), s), z), 0.0f);
+                const float t1 = __fadd_rn(__fadd_rn(__fdiv_rn(P::hi(w[j]), s), z), 0.0f);
                 word |= f32x2_to_e2m1x2(t0, t1) << (8 * j);
             }
             o[k] = word;
@@ -168,8 +170,9 @@ struct Fp4NvQuantPackOp {
         bool slow = false;
 #pragma unroll
         for (int g = 0; g < 2; ++g) {
-            const float a = fabsf(s[g]);
-            slow |= !(a >= 7.888609052210118e-31f && a <= 1024.0f);   // [2^-100, 2^10]; NaN -> slow
+            // [2^-100, 2^10]; a negative or NaN scale goes slow too: under a negative s the residual step turns x = +0.0 into -0.0,
+            // where the reference's torch.sign gives +0.0
+            slow |= !(s[g] >= 7.888609052210118e-31f && s[g] <= 1024.0f);
             rc[g] = __frcp_rn(s[g]);
             // zero_point.to(x.dtype): fp8 / small integers are exact in bf16 and fp16
             z[g] = fp4_zp_value<ZK>(r.z >> (8 * g));
@@ -239,7 +242,7 @@ struct Fp4NvObserveQuantPackOp {
         uint32_t codes;
     };
     // out of line, everything by value: a unit with a group outside the ranges the shortcuts are proven for (max |x| above 2^14 or
-    // below 2^-40, a global scale outside [2^-60, 2^60], an effective scale outside [2^-100, 2^10], NaN) -> IEEE division everywhere
+    // below 2^-40, a global scale outside [2^-60, 2^60], an effective scale outside [2^-100, 2^10] or negative, NaN) -> IEEE division everywhere
     __device__ static __noinline__ SlowOut unit_slow_observe(uint4 c0, uint4 c1, uint4 c2, uint4 c3, float amax0, float amax1, float gs, int off) {
         using Q = Fp4NvQuantPackOp<P, FS_F32, FZ_NONE>;
         uint32_t b0, b1;
@@ -273,8 +276,7 @@ struct Fp4NvObserveQuantPackOp {
             codes |= byte << (8 * g);
             // scale / global_scale: an e4m3 value (within [2^-9, 448]) over the global scale, same shortcut as the decompress kernel
             s[g] = recip_div(sf, tc.gs, tc.rgs);
-            const float a = fabsf(s[g]);
-            slow |= !(a >= 7.888609052210118e-31f && a <= 1024.0f);                     // [2^-100, 2^10]; NaN -> slow
+            slow |= !(s[g] >= 7.888609052210118e-31f && s[g] <= 1024.0f);                // [2^-100, 2^10]; negative (gs < 0), NaN -> slow
             rc[g] = __frcp_rn(s[g]);
         }
         uint32_t o[4];
