@@ -104,6 +104,8 @@ class HadamardJob(ctypes.Structure):
         ("precision", ctypes.c_int32),
         ("log2_n", ctypes.c_int32),
         ("inverse", ctypes.c_int32),
+        ("core", ctypes.c_void_p),
+        ("core_order", ctypes.c_int32),
     ]
 
 

@@ -178,13 +178,17 @@ int cpu_run_one(int op, const ct_quant_desc& d, const void* in, const void* scal
     return CT_E_UNSUPPORTED;
 }
 
-// ct_hadamard_transform on the host: the butterfly order of hadamard.cu (stage h = 1, 2, ..., n/2), the same conversions (hadamard.cuh)
+// ct_hadamard_transform on the host: the butterfly order of hadamard.cu (stage h = 1, 2, ..., 2^log2_n / 2), the core stage's sequential
+// sums over a = 0 .. K - 1, the same conversions (hadamard.cuh)
 template <class C, int DT>
 static void cpu_hadamard_rows(const ct_hadamard_job& j) {
     using E = Elem<DT>;
     using T = typename E::T;
-    const int64_t n = (int64_t)1 << j.log2_n;
-    const int64_t per_row = j.shape[3] >> j.log2_n;
+    const int64_t m = (int64_t)1 << j.log2_n;
+    const int64_t K = j.core_order > 0 ? j.core_order : 1;
+    const int64_t n = K * m;
+    const bool mix = j.core_order > 0 && j.core != nullptr;
+    const int64_t per_row = j.shape[3] / n;
     const int64_t rows = j.shape[0] * j.shape[1] * j.shape[2] * per_row;
     const C scale = (C)std::sqrt((double)n);
     const T* x = reinterpret_cast<const T*>(j.x);
@@ -192,6 +196,7 @@ static void cpu_hadamard_rows(const ct_hadamard_job& j) {
 #pragma omp parallel
     {
         C* z = new C[n];
+        C* y = new C[n];
 #pragma omp for schedule(static)
         for (int64_t r = 0; r < rows; ++r) {
             const int64_t bhs = r / per_row, k = r % per_row;
@@ -204,13 +209,26 @@ static void cpu_hadamard_rows(const ct_hadamard_job& j) {
                 if (j.sign && !j.inverse && j.sign[q] < 0) v = -v;
                 z[q] = v;
             }
-            for (int64_t hh = 1; hh < n; hh <<= 1)
+            for (int64_t hh = 1; hh < m; hh <<= 1)
                 for (int64_t i = 0; i < n; ++i)
                     if (!(i & hh)) {
                         const C a = z[i], c = z[i + hh];
                         z[i] = a + c;
                         z[i + hh] = a - c;
                     }
+            if (mix) {
+                for (int64_t c = 0; c < K; ++c)
+                    for (int64_t d = 0; d < m; ++d) {
+                        C acc = 0;
+                        for (int64_t a = 0; a < K; ++a) {
+                            const bool neg = (j.inverse ? j.core[a * K + c] : j.core[c * K + a]) < 0;
+                            const C v = z[a * m + d];
+                            acc = a == 0 ? (neg ? -v : v) : (neg ? acc - v : acc + v);
+                        }
+                        y[c * m + d] = acc;
+                    }
+                std::memcpy(z, y, sizeof(C) * n);
+            }
             for (int64_t i = 0; i < n; ++i) {
                 const int64_t q = j.perm ? j.perm[i] : i;
                 C v = z[q];
@@ -219,6 +237,7 @@ static void cpu_hadamard_rows(const ct_hadamard_job& j) {
             }
         }
         delete[] z;
+        delete[] y;
     }
 }
 

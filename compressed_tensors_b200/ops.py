@@ -605,9 +605,10 @@ def dynamic_fake_quantize(x: torch.Tensor, args, global_scale: Optional[torch.Te
 # Walsh-Hadamard transforms (transform/factory/hadamard.py, HadamardTransform.forward)
 # --------------------------------------------------------------------------------------------
 HADAMARD_MAX_ORDER = 1 << 15
+HADAMARD_MAX_CORE = 256
 
 
-def _hadamard_job(x: torch.Tensor, out: torch.Tensor, log2_n: int, sign, perm, inverse: bool, precision) -> N.HadamardJob:
+def _hadamard_job(x: torch.Tensor, out: torch.Tensor, log2_n: int, sign, perm, inverse: bool, precision, core=None) -> N.HadamardJob:
     j = N.HadamardJob()
     j.x, j.out = x.data_ptr(), out.data_ptr()
     j.shape[:] = list(x.shape)
@@ -617,6 +618,8 @@ def _hadamard_job(x: torch.Tensor, out: torch.Tensor, log2_n: int, sign, perm, i
     j.dtype = N.DT[x.dtype]
     j.precision = N.DT_F64 if precision == torch.float64 else N.DT[torch.float32]
     j.log2_n, j.inverse = log2_n, int(bool(inverse))
+    if core is not None:
+        j.core, j.core_order = core.data_ptr(), core.size(0)
     return j
 
 
@@ -640,9 +643,30 @@ def _verified_permutation(perm: torch.Tensor, n: int) -> torch.Tensor:
     return checked
 
 
+def _verified_core(core: torch.Tensor, n: int) -> torch.Tensor:
+    """core must be a K x K matrix of +-1 values with n = K * 2^m.  Returns an int8 copy made when it was checked, once per version
+    and storage of the tensor, as _verified_permutation does for perm."""
+    if core.ndim != 2 or core.size(0) != core.size(1) or core.size(0) < 1 or core.size(0) > HADAMARD_MAX_CORE:
+        raise ValueError(f"core must be a square matrix of order 1 .. {HADAMARD_MAX_CORE}, got shape {tuple(core.shape)}")
+    k = core.size(0)
+    if n % k or (n // k) & (n // k - 1):
+        raise ValueError(f"the order {n} is not {k} * 2^m for the core of order {k}")
+    if core.device.type == "meta":
+        return core
+    key = (core._version, core.data_ptr())
+    cached = getattr(core, "_ct_checked_core", None)
+    if cached is not None and cached[0] == key:
+        return cached[1]
+    if core.is_complex() or core.dtype == torch.bool or not bool(((core == 1) | (core == -1)).all()):
+        raise ValueError("core must hold +-1 values only")
+    checked = core.detach().to(torch.int8, copy=True).contiguous()
+    core._ct_checked_core = (key, checked)
+    return checked
+
+
 @torch.no_grad()
 def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = None, perm: Optional[torch.Tensor] = None,
-                       inverse: bool = False, precision: torch.dtype = torch.float32) -> torch.Tensor:
+                       inverse: bool = False, precision: torch.dtype = torch.float32, core: Optional[torch.Tensor] = None) -> torch.Tensor:
     """
     `(x.to(precision) @ M / sqrt(n)).to(x.dtype)` along the last dimension, block-diagonal over its n-element blocks, for the structured
     matrices of the `hadamard` / `random-hadamard` factories: M = H (Sylvester), with rows and columns permuted by `perm` (a permutation
@@ -652,12 +676,22 @@ def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = N
     tensor's next tracked write.  An O(n log n) butterfly
     (ct_hadamard_transform) instead of the dense product; precision fp32 or fp64.  The output has x's strides when x is dense (the
     transposed [B, H, S, D] attention states included), so no contiguous copy is made in or out.
+
+    `core` (a K x K tensor of +-1 values, int8 or float) replaces H by (C ⊗ H_{2^m})^T for n = K * 2^m, the matrices the reference's
+    random_hadamard_matrix builds for orders that are not powers of two: the butterflies run on each 2^m slice and the K slices are
+    mixed with C (K additions per element).  A core that is not square, not +-1 or whose order K does not give n = K * 2^m raises
+    ValueError; it is checked once per version of the tensor, like `perm`.
     """
     n = int(n)
-    if n <= 0 or n & (n - 1):
-        raise ValueError("Cannot construct deterministic hadamard of size != 2^n")
-    if n > HADAMARD_MAX_ORDER or n < 2:
-        raise NotImplementedError(f"hadamard_transform covers orders 2 .. {HADAMARD_MAX_ORDER}, got {n}")
+    if core is not None:
+        if n > HADAMARD_MAX_ORDER:
+            raise NotImplementedError(f"hadamard_transform covers orders up to {HADAMARD_MAX_ORDER}, got {n}")
+        core = _verified_core(core, n)
+    else:
+        if n <= 0 or n & (n - 1):
+            raise ValueError("Cannot construct deterministic hadamard of size != 2^n")
+        if n > HADAMARD_MAX_ORDER or n < 2:
+            raise NotImplementedError(f"hadamard_transform covers orders 2 .. {HADAMARD_MAX_ORDER}, got {n}")
     _check_float(x, "input")
     if precision not in (torch.float32, torch.float64):
         raise NotImplementedError(f"hadamard_transform computes in float32 or float64, got {precision}")
@@ -682,12 +716,13 @@ def hadamard_transform(x: torch.Tensor, n: int, sign: Optional[torch.Tensor] = N
         out = torch.empty_like(v)
     sg = _to_dev(torch.where(sign < 0, -1, 1).to(torch.int8) if sign is not None and sign.dtype != torch.int8 else sign, idx)
     pm = _to_dev(perm, idx)
-    log2_n = n.bit_length() - 1
-    rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision)), idx, _stream(idx))
+    cr = _to_dev(core, idx)
+    log2_n = (n // core.size(0) if core is not None else n).bit_length() - 1
+    rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision, cr)), idx, _stream(idx))
     if rc == N.CT_E_UNSUPPORTED and not v.is_contiguous():
         v = v.contiguous()
         out = torch.empty_like(v)
-        rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision)), idx, _stream(idx))
+        rc = N.lib().ct_hadamard_transform(ctypes.byref(_hadamard_job(v, out, log2_n, sg, pm, inverse, precision, cr)), idx, _stream(idx))
     N.check(rc, "hadamard_transform")
     return _back(out.view(x.shape), x)
 

@@ -4,7 +4,9 @@ The `hadamard` factory (the reference's transform/factory/hadamard.py).
 A HadamardTransform holds the dense matrix (`weight`, n x n, in the scheme's precision, float64 for the weight locations) and, with
 `randomize`, the permutation `perm`, exactly as the reference does, so state dicts and checkpoints are the same.  Its forward runs
 the Walsh-Hadamard kernel (`ops.hadamard_transform`) when `weight` is verified to be diag(Q) . H with H Sylvester's matrix (Q is
-read from the first column; the whole matrix is checked once per parameter version, and Q and perm are kept on the device of use);
+read from the first column; the whole matrix is checked once per parameter version, and Q and perm are kept on the device of use).
+Otherwise, for an order n = K * 2^m of the reference's table (K as the reference chooses it), it tries the reference's
+random-hadamard structure diag(s) . (C ⊗ H_{2^m})^T with a K x K +-1 core C, read off the weight and passed to the kernel as `core`;
 a trained weight (`requires_grad`), any other matrix, another precision, or an input that needs autograd runs the reference's dense
 formula.
 """
@@ -18,7 +20,7 @@ from ... import ops
 from ...offload import get_execution_device
 from ...utils.helpers import ParameterizedDefaultDict
 from .. import TransformArgs, TransformLocation, TransformScheme
-from ..utils.hadamard import deterministic_hadamard_matrix, is_pow2
+from ..utils.hadamard import deterministic_hadamard_matrix, is_pow2, table_core_order
 from ..utils.matrix import apply_transform_weight, get_transform_size
 from .base import TransformBase, TransformFactory
 
@@ -98,7 +100,7 @@ class HadamardTransform(TransformBase):
         out = apply_transform_weight(weight.to(device=value.device), value.to(dtype=weight.dtype), self.args.location, self.module_type)
         return (out / self._scale).to(value.dtype)
 
-    def _kernel(self, value: Tensor, sign: Tensor | None, perm: Tensor | None) -> Tensor:
+    def _kernel(self, value: Tensor, sign: Tensor | None, perm: Tensor | None, core: Tensor | None = None) -> Tensor:
         """the same product as _dense through the butterfly: rows of `value` (or of value^T) times M or M^T"""
         n, inverse, location = self.weight.size(0), bool(self.args.inverse), TransformLocation(self.args.location)
         columns = False
@@ -114,30 +116,35 @@ class HadamardTransform(TransformBase):
         x = value.T if columns else value
         if x.ndim == 0 or x.shape[-1] % n:
             return self._dense(value)
-        y = ops.hadamard_transform(x, n, sign, perm, inverse, self.weight.dtype)
+        y = ops.hadamard_transform(x, n, sign, perm, inverse, self.weight.dtype, core=core)
         return y.T if columns else y
 
 
 def _structured_signs(weight: Tensor, perm: Tensor | None, value: Tensor):
-    """(sign, perm) on value's device when the kernel computes exactly the product the dense formula asks for, else None"""
+    """(sign, perm, core) on value's device when the kernel computes exactly the product the dense formula asks for, else None"""
     if (weight.requires_grad or weight.device.type == "meta" or value.device.type == "meta" or weight.dtype not in (torch.float32, torch.float64)
             or value.dtype not in (torch.float32, torch.float16, torch.bfloat16) or (torch.is_grad_enabled() and value.requires_grad)):
         return None
     n = weight.size(0)
     if n > ops.HADAMARD_MAX_ORDER:
         raise NotImplementedError(f"Hadamard transforms of order {n} > {ops.HADAMARD_MAX_ORDER} are not supported")
-    if n < 2 or weight.ndim != 2 or weight.size(1) != n or not is_pow2(n):
+    if n < 2 or weight.ndim != 2 or weight.size(1) != n:
         return None
-    entry = _verified(weight, "_ct_hadamard_signs", _sign_vector)
-    if entry is None:
-        return None
-    sign = _on(entry, value.device)
+    core = None
+    entry = _verified(weight, "_ct_hadamard_signs", _sign_vector) if is_pow2(n) else None
+    if entry is not None:
+        sign = _on(entry, value.device)
+    else:
+        entry = _verified(weight, "_ct_hadamard_core", _core_factors) if table_core_order(n) is not None else None
+        if entry is None:
+            return None
+        sign, core = _on(entry, value.device)
     if perm is None:
-        return sign, None
+        return sign, None, core
     pentry = _verified(perm, "_ct_hadamard_perm", lambda p: p.clone() if p.ndim == 1 and p.numel() == n and _is_permutation(p) else None)
     if pentry is None:
         return None
-    return sign, _on(pentry, value.device)
+    return sign, _on(pentry, value.device), core
 
 
 def _verified(t: Tensor, attr: str, check):
@@ -160,7 +167,7 @@ def _on(entry, dev: torch.device):
     if result is True:          # Sylvester's matrix itself: no signs
         return None
     if dev not in copies:
-        copies[dev] = result.to(dev)
+        copies[dev] = tuple(t.to(dev) for t in result) if isinstance(result, tuple) else result.to(dev)
     return copies[dev]
 
 
@@ -181,6 +188,39 @@ def _sign_vector(w: Tensor):
         if not torch.equal(w[r0:r0 + block], expected):
             return None
     return True if bool((q == 1).all()) else q.to(torch.int8).contiguous()   # w is fp32 / fp64: .to(int8) is a copy
+
+
+def _parity_signs(rows: Tensor, cols: Tensor, dtype: torch.dtype) -> Tensor:
+    """H[rows][:, cols] of Sylvester's matrix, (-1)^popcount(r & c)"""
+    p = rows[:, None] & cols[None, :]
+    for s in (8, 4, 2, 1):
+        p = p ^ (p >> s)
+    return (1 - 2 * (p & 1)).to(dtype)
+
+
+def _core_factors(w: Tensor):
+    """(s, C) as int8 when w = diag(s) . (C ⊗ H_{2^m})^T, the reference's random-hadamard matrix, with C of the order K its table
+    gives for n = K * 2^m, else None.  The row signs and C are determined up to a sign per row block a; the rule fixed here takes
+    s = w[:, 0] and C[c][a] = w[a 2^m][c 2^m] s[a 2^m] (so C[0][:] = 1).  The whole matrix is checked against them in row blocks."""
+    n = w.size(0)
+    k = table_core_order(n)
+    m = n // k
+    s = w[:, 0]
+    if not bool(((s == 1) | (s == -1)).all()):
+        return None
+    core = (w[::m, ::m] * s[::m, None]).T.contiguous()
+    if not bool(((core == 1) | (core == -1)).all()):
+        return None
+    log2_m = m.bit_length() - 1
+    cols = torch.arange(n, device=w.device)
+    block = max(1, (1 << 22) // n)
+    for r0 in range(0, n, block):
+        rows = torch.arange(r0, min(n, r0 + block), device=w.device)
+        expected = (_parity_signs(rows & (m - 1), cols & (m - 1), w.dtype) * core[(cols >> log2_m)[None, :], (rows >> log2_m)[:, None]]
+                    * s[r0:r0 + block, None])
+        if not torch.equal(w[r0:r0 + block], expected):
+            return None
+    return s.to(torch.int8).contiguous(), core.to(torch.int8)
 
 
 def _is_permutation(p: Tensor) -> bool:

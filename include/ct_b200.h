@@ -166,7 +166,12 @@ int ct_fake_quantize_heads(int n, const ct_head_job* jobs, int device, void* str
  * one conversion to `dtype` (fp64 reaches 16-bit dtypes through fp32, as torch's CPU conversion does).  x and out are [B, H, S, D]
  * views with the same element strides (stride[3] == 1; anything else returns CT_E_UNSUPPORTED: run it on a contiguous copy); sign is
  * int8 +-1 [n] or NULL, perm int64 [n] or NULL, both on the device of x.  device = CT_DEVICE_CPU runs the host twin (same butterfly
- * order, same bits) on host pointers.  Enqueue-only on a device. */
+ * order, same bits) on host pointers.  Enqueue-only on a device.
+ * With core_order = K >= 1, n = K . 2^log2_n (0 <= log2_n, n <= 2^15) and H above is (C (x) H_{2^log2_n})^T, C = `core` (K x K, +-1):
+ * the matrices the reference's random_hadamard_matrix builds from its table of known Hadamard matrices.  The butterflies run on each
+ * 2^log2_n slice, then the K slices are mixed with C (C^T under `inverse`), summing sequentially over the K rows; K additions per
+ * element.  CT_E_SHAPE for K outside 1 .. 256 or n above 2^15, CT_E_ARG for a NULL core with K > 1 (K = 1 and NULL: C = [1]).
+ * Zero-initialised core fields (core_order 0) leave the forms above unchanged. */
 typedef struct ct_hadamard_job {
     const void* x;
     void* out;
@@ -178,6 +183,8 @@ typedef struct ct_hadamard_job {
     int32_t precision;      /* CT_F32 / CT_F64 */
     int32_t log2_n;
     int32_t inverse;
+    const int8_t* core;     /* K x K +-1, row-major, on the device of x; NULL with core_order 0 or 1 */
+    int32_t core_order;     /* K: 0 = no core (the forms above) */
 } ct_hadamard_job;
 int ct_hadamard_transform(const ct_hadamard_job* job, int device, void* stream);
 

@@ -156,7 +156,7 @@ def batched_family(dt):
 def transform_family(dt):
     """ct_hadamard_transform: every order in both precisions with one-row partial last tiles, fp64 at 2^15 on more tiles than its
     grid of 2 x SMs (CTAs reuse their global scratch slice), rows one element off alignment (element loads and stores) with sign,
-    perm and inverse, and strided [B, H, S, D] views with head blocking and decode"""
+    perm and inverse, and strided [B, H, S, D] views with head blocking and decode; the same with a core of orders 12 .. 256"""
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
     for log2_n in range(1, 16):
         n = 1 << log2_n
@@ -175,6 +175,23 @@ def transform_family(dt):
         q = (torch.randint(0, 2, (n,), device=DEV) * 2 - 1).to(torch.int8)
         for precision in (torch.float32, torch.float64):
             ops.hadamard_transform(x, n, q, torch.randperm(n, device=DEV), True, precision)
+    # with a K x K core (n = K * 2^m): partial last tiles, persistent CTAs over more tiles than the grid, the fp64 scratch tiles at
+    # n = 224 * 128, unaligned rows and a strided view
+    for k, m in ((12, 1), (20, 4), (172, 64), (224, 64), (224, 128), (256, 128)):
+        n = k * m
+        core = (torch.randint(0, 2, (k, k), device=DEV) * 2 - 1).to(torch.int8)
+        rows = 8 * sms + 5 if n == 224 * 64 else (2 * sms + 7 if n > 25600 else 4096 // n + 1)
+        x = torch.randn(rows, n, device=DEV).to(dt)
+        q = (torch.randint(0, 2, (n,), device=DEV) * 2 - 1).to(torch.int8)
+        perm = torch.randperm(n, device=DEV)
+        odd = torch.randn(3 * n + 1, device=DEV).to(dt)[1:].view(3, n)
+        for precision in (torch.float32, torch.float64):
+            for sign, p, inverse in ((None, None, False), (q, perm, False), (q, perm, True)):
+                ops.hadamard_transform(x, n, sign, p, inverse, precision, core=core)
+                ops.hadamard_transform(odd, n, sign, p, inverse, precision, core=core)
+        if n <= 4096:
+            v = torch.randn(2, 9, 3, 2 * n, device=DEV).to(dt).transpose(1, 2)
+            ops.hadamard_transform(v, n, q, perm, True, torch.float32, core=core)
 
 
 def heads_family(dt):
