@@ -14,6 +14,7 @@ import torch
 from torch.nn import Module
 
 from ... import ops
+from ...offload.cache import OffloadCache
 from ..quant_args import DynamicType, QuantizationArgs
 from ..quant_config import QuantizationStatus
 from ..quant_scheme import QuantizationScheme
@@ -85,6 +86,11 @@ def set_forward_quantized(module: torch.nn.Linear | torch.nn.Embedding):
 
     @wraps(original)
     def quantized_forward(self, input: torch.Tensor) -> torch.Tensor:
+        if isinstance(self._parameters, OffloadCache) and not OffloadCache.offloading_disabled:
+            # an offloaded weight is onloaded anew on every read: keep the first onloaded copy for the whole call, so that the
+            # layer's own forward reads the fake-quantized data patched into it (the reference loses it here)
+            with OffloadCache.disable_offloading():
+                return quantized_forward(self, input)
         scheme: QuantizationScheme | None = getattr(self, "quantization_scheme", None)
         status: QuantizationStatus | None = getattr(self, "quantization_status", None)
         enabled = getattr(self, "quantization_enabled", True) and scheme is not None and status is not None

@@ -13,6 +13,7 @@ import math
 import torch
 from torch.nn import Module, Parameter
 
+from ...offload import OffloadCache, get_execution_device, unwrap_offload_forward
 from ...utils.helpers import deprecated, get_head_dim, get_num_attn_heads, get_num_kv_heads
 from ..quant_args import ActivationOrdering, DynamicType, QuantizationArgs, QuantizationStrategy
 from ..quant_config import QuantizationStatus
@@ -52,7 +53,8 @@ def initialize_module_for_quantization(module: Module, scheme: QuantizationSchem
             initialize_qparams(module, "weight", scheme.weights, weight.shape, weight.dtype, force_zero_point)
         if scheme.output_activations is not None:
             initialize_qparams(module, "output", scheme.output_activations, weight.shape[:-1], weight.dtype, force_zero_point)
-        set_forward_quantized(module)
+        with unwrap_offload_forward(module):   # an offloaded module keeps moving its inputs to the onload device
+            set_forward_quantized(module)
     else:
         raise ValueError(f"Quantization of module type {type(module)} is not supported")
     module.quantization_scheme = scheme
@@ -118,7 +120,9 @@ def initialize_attn_qparams(module: Module, scheme: QuantizationScheme, force_ze
 def initialize_qparams(module: Module, base_name: str, quantization_args: QuantizationArgs, observed_shape, observed_dtype: torch.dtype,
                        force_zero_point: bool = True):
     strategy, dynamic = quantization_args.strategy, quantization_args.dynamic
-    if getattr(module, "weight", None) is not None:
+    if isinstance(module._parameters, OffloadCache):
+        device = get_execution_device(module)   # created where the module runs, then offloaded by its cache
+    elif getattr(module, "weight", None) is not None:
         device = module.weight.device
     else:   # attention modules: the device of their projections
         device = next(module.parameters(), torch.empty(0)).device

@@ -19,7 +19,7 @@ from torch.nn import Module, Parameter
 from ...distributed import is_distributed
 from ...modeling.attention import initialize_hooked_attention, register_query_hook
 from ...modeling.kvcache import initialize_hooked_kv_cache, register_key_hook
-from ...offload import OffloadCache, update_offload_parameter
+from ...offload import OffloadCache, align_module_device, register_offload_module, update_offload_parameter
 from ...registry.registry import RegistryMixin
 from ...utils.helpers import patch_attr
 from ...utils.internal import InternalModule
@@ -74,7 +74,7 @@ class TransformFactory(RegistryMixin, ABC):
         """create the transform of `module` for `args` and apply it at its location"""
         transform_name = f"{self.name}_{args.location}"
         transform = self.create_transform(module, args)
-        module.register_module(transform_name, transform)
+        register_offload_module(module, transform_name, transform)   # offloaded like `module` when it is offloaded
 
         if args.location == TransformLocation.INPUT:
 
@@ -85,7 +85,8 @@ class TransformFactory(RegistryMixin, ABC):
 
         elif args.location in (TransformLocation.WEIGHT_INPUT, TransformLocation.WEIGHT_OUTPUT):
             assert hasattr(module, "weight")
-            with torch.no_grad():
+            # an offloaded module's weight is onloaded once, fused on the onload device and written back to its cache
+            with torch.no_grad(), align_module_device(module):
                 update_offload_parameter(module, "weight", transform(module.weight))
                 # y' = R (W x + b) = (R W) x + R b: a rotated output needs the rotated bias too
                 if args.location == TransformLocation.WEIGHT_OUTPUT and getattr(module, "bias", None) is not None:
