@@ -1228,8 +1228,9 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
     fused kernel; returns (codes or packed words, scale, zero point or None) exactly as the reference's
     min/max -> calculate_qparams (utils/helpers.py:50-137) -> quantize(dtype=args.pytorch_dtype()) [-> pack_to_int32] flow does.
 
-      CHANNEL (one scale per row): bf16 / fp16, cols % 8 == 0, cols <= 16384 -> `ct_observe_quantize_channel`
-                                   (int8 codes, float8_e4m3fn codes, or 4- / 8-bit packed int32)
+      CHANNEL (one scale per row): bf16 / fp16, cols % 8 == 0 -> `ct_observe_quantize_channel` (int8 codes, float8_e4m3fn codes,
+                                   or 4- / 8-bit packed int32); one CTA per row up to 16384 columns, one thread-block cluster per row
+                                   up to 131072; wider rows are declined by the kernel and take the unfused path below
       TENSOR (one scale)         : `ct_observe_quantize_tensor` -- grid-wide min / max, calculate_qparams by the last CTA, then the
                                    streaming quantize kernel with the device-resident scale; no host round trip (the FP8 preset)
       GROUP + pack               : `observe_quantize_pack`
@@ -1253,7 +1254,7 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
     idx = _dev_index(x)
     xd = _to_dev(x, idx).contiguous()
     qdt = torch.int32 if pack else (torch.float8_e4m3fn if qtype == N.Q_FLOAT else torch.int8)
-    fused_ok = (strategy == "channel" and x.dtype in (torch.bfloat16, torch.float16) and cols % 8 == 0 and 0 < cols <= 16384 and rows > 0
+    fused_ok = (strategy == "channel" and x.dtype in (torch.bfloat16, torch.float16) and cols % 8 == 0 and cols > 0 and rows > 0
                 and qtype in (N.Q_INT, N.Q_FLOAT) and (bits in (4, 8) if pack else bits == 8) and (symmetric or qtype == N.Q_INT))
     if fused_ok:
         scale = torch.empty((rows, 1), dtype=x.dtype, device=xd.device)
@@ -1265,8 +1266,9 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
         d.zp_dtype = N.DT_NONE if symmetric else N.DT[torch.int8]
         d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT[qdt], N.DT_NONE, qtype, bits
         rc = N.lib().ct_observe_quantize_channel(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(out), idx, N.stream_ptr(idx))
-        N.check(rc, "observe_quantize")
-        return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+        if rc != N.CT_E_UNSUPPORTED:   # declined (a row wider than one cluster holds): the unfused path below
+            N.check(rc, "observe_quantize")
+            return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
     if (strategy == "tensor" and _tensor_observer_ok(xd) and qtype in (N.Q_INT, N.Q_FLOAT) and (symmetric or qtype == N.Q_INT)
             and (bits in (4, 8) if pack else bits == 8) and (not pack or (cols * bits) % 32 == 0)):
         # ONE call: grid-wide min / max -> calculate_qparams on the device -> quantize (or quantize + pack) with the device-resident scale
