@@ -51,7 +51,8 @@ __global__ void __launch_bounds__(256) awq_repack_kernel(const uint32_t* __restr
 #pragma unroll
         for (int j = 0; j < 8; ++j) r[j] = tile[j][nl];
         uint32_t* dst_row = out + n * KW + kw0;
-        if (kw0 + 8 <= KW && (KW % 4) == 0) {
+        // uint4 stores need a 16-byte aligned row: KW % 4 == 0 aligns every row to the base, which must be aligned itself
+        if (kw0 + 8 <= KW && (KW % 4) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0) {
             reinterpret_cast<uint4*>(dst_row)[0] = make_uint4(r[0], r[1], r[2], r[3]);
             reinterpret_cast<uint4*>(dst_row)[1] = make_uint4(r[4], r[5], r[6], r[7]);
         } else {
