@@ -7,6 +7,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstring>
+#include <vector>
+
 #include "../../include/ct_b200.h"
 
 namespace ctb {
@@ -29,6 +32,39 @@ constexpr int GRID_SMS = 132;   // SMs of an H100 SXM: grid size of the grid-str
 int sm_count(int device);
 int64_t l2_bytes(int device);   // L2 cache size of the device (0 when unknown)
 int scratch_alloc(void** p, size_t bytes, int device, cudaStream_t stream);   // stream-ordered, free with cudaFreeAsync
+
+// Job tables of multi-job launches normally reach the device with one cudaMemcpyAsync from a host image -- a pageable-memory copy,
+// which a stream capture rejects.  While the stream is being captured the table travels as KERNEL PARAMETERS instead (PER jobs per
+// launch of a one-warp kernel; parameters are copied into the graph node at capture time), so a whole-model call can be captured
+// once and replayed.
+template <class J, int PER> struct JobBlock { J j[PER]; };
+template <class J, int PER>
+__global__ void upload_jobs_kernel(J* dst, const __grid_constant__ JobBlock<J, PER> blk, int n) {
+    if ((int)threadIdx.x < n) dst[threadIdx.x] = blk.j[threadIdx.x];
+}
+// writes `head` zero bytes at dst, then jobs[0, n) (device memory, stream-ordered)
+template <class J, int PER>
+int upload_jobs(uint8_t* dst, size_t head, const J* jobs, size_t n, cudaStream_t stream) {
+    static_assert(PER <= 32, "one thread per job of a block");
+    cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(stream, &capturing);
+    if (capturing == cudaStreamCaptureStatusActive) {
+        if (head) CT_CUDA_TRY(cudaMemsetAsync(dst, 0, head, stream));
+        for (size_t o = 0; o < n; o += PER) {
+            JobBlock<J, PER> blk;
+            const int cnt = (int)(n - o < (size_t)PER ? n - o : PER);
+            memcpy(blk.j, jobs + o, (size_t)cnt * sizeof(J));
+            upload_jobs_kernel<J, PER><<<1, 32, 0, stream>>>(reinterpret_cast<J*>(dst + head) + o, blk, cnt);
+        }
+        count_launch((int)((n + PER - 1) / PER));
+        CT_CUDA_TRY(cudaGetLastError());
+        return CT_OK;
+    }
+    std::vector<uint8_t> img(head + n * sizeof(J), 0);
+    memcpy(img.data() + head, jobs, n * sizeof(J));
+    CT_CUDA_TRY(cudaMemcpyAsync(dst, img.data(), img.size(), cudaMemcpyHostToDevice, stream));
+    return CT_OK;
+}
 
 // RAII device guard
 struct DeviceGuard {

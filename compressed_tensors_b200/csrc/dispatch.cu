@@ -38,21 +38,34 @@ static int validate_desc(const ct_quant_desc* d) {
     return CT_OK;
 }
 
-// Job tables of multi-tensor launches normally reach the device with one cudaMemcpyAsync from a host image -- a pageable-memory copy,
-// which a stream capture rejects.  While the stream is being captured the table travels as KERNEL PARAMETERS instead (32 jobs = 3.3 KB
-// per launch of this one-warp kernel; parameters are copied into the graph node at capture time), so a whole-model ct_batched call can
-// be captured once and replayed.
-struct JobBlock { Job j[32]; };
-static __global__ void upload_jobs_kernel(Job* dst, const __grid_constant__ JobBlock blk, int n) {
-    if ((int)threadIdx.x < n) dst[threadIdx.x] = blk.j[threadIdx.x];
-}
-
 struct Plan {
-    bool fast;
-    FastSig sig;
-    Job job;        // tile_begin/end filled by the caller
+    StreamKernel k;   // k.launch == nullptr: the tensor takes the generic kernels
+    Job job;          // tile_begin/end filled by the caller
     Common cm;
 };
+
+// The streaming plan of kernel k (none: the generic plan) over n elements in chunks of `chunk`, D elements per scale element;
+// `two_d`: the 2-D scale addressing of d (BLOCK strategy, one-row group scales).
+static Plan fast_plan(StreamKernel k, const Common& cm, const void* in, const void* scale, const void* zp, void* out, const void* aux,
+                      int64_t n, int64_t chunk, int64_t D, const ct_quant_desc* two_d = nullptr) {
+    Plan p{};
+    if (!k.launch) return p;
+    p.k = k;
+    p.cm = cm;
+    p.job.in = reinterpret_cast<const uint8_t*>(in);
+    p.job.scale = scale;
+    p.job.zp = zp;
+    p.job.out = reinterpret_cast<uint8_t*>(out);
+    p.job.aux = aux;
+    p.job.n_chunks = (uint32_t)(n / chunk);
+    p.job.dc = make_fastdiv(is_inf(D) ? (uint64_t)0x7FFFFFFFull : (uint64_t)(D / chunk));
+    if (two_d) {
+        p.job.cpr = make_fastdiv((uint64_t)(two_d->cols / chunk));
+        p.job.rd = make_fastdiv(is_inf(two_d->rdiv) ? (uint64_t)0x7FFFFFFFull : (uint64_t)two_d->rdiv);
+        p.job.srs = (uint32_t)two_d->s_row_stride;
+    }
+    return p;
+}
 
 static uint32_t bits_of(int dt, float v) {
     // v as a 16-bit float pattern duplicated in both halves (host-side conversion, RNE; v is exact)
@@ -91,124 +104,88 @@ Common make_common(int p_dt, int qtype, int bits) {
 // Try to express (op, desc) as a streaming job.  in/out are the streamed tensors of the op.
 static Plan plan_one(int op, const ct_quant_desc& d, const void* in, const void* scale, const void* zp,
                      const int32_t* g_idx, void* out) {
-    Plan p;
-    p.fast = false;
-    memset(&p.job, 0, sizeof(p.job));
-    memset(&p.cm, 0, sizeof(p.cm));
-    p.sig = FastSig{0, 0, 0, 0, 1};
     const int64_t n = d.rows * d.cols;
-    if (g_idx || n == 0 || n % 8 != 0 || (n / 8) >= 0x7fffffffLL) return p;
-    if (!aligned16(in) || !aligned16(out)) return p;
-    if (d.global_scale || d.qtype == CT_Q_FP4) return p;   // two-level scales / FP4 rounding: fp4 ops have their own plans (below), the rest is generic
+    if (g_idx || n == 0 || n % 8 != 0 || (n / 8) >= 0x7fffffffLL) return {};
+    if (!aligned16(in) || !aligned16(out)) return {};
+    if (d.global_scale || d.qtype == CT_Q_FP4) return {};   // two-level scales / FP4 rounding: fp4 ops have their own plans (below), the rest is generic
     int64_t D;
     bool two_d = false;
     if (!flat_divisor(d, D)) {
         // 2-D scale addressing (BLOCK strategy, one-row group scales): chunks must not straddle rows or column blocks
-        if (op == CT_OP_OBSERVE_QUANTIZE_PACK || d.cols % 8 != 0 || (d.cols / 8) >= 0x7fffffffLL) return p;
-        if (!is_inf(d.cdiv) && d.cdiv % 8 != 0) return p;
-        if (d.s_row_stride < 0 || d.s_row_stride >= 0x7fffffffLL) return p;
+        if (op == CT_OP_OBSERVE_QUANTIZE_PACK || d.cols % 8 != 0 || (d.cols / 8) >= 0x7fffffffLL) return {};
+        if (!is_inf(d.cdiv) && d.cdiv % 8 != 0) return {};
+        if (d.s_row_stride < 0 || d.s_row_stride >= 0x7fffffffLL) return {};
         two_d = true;
         D = d.cdiv;
     }
-    if (!is_inf(D) && D % 8 != 0) return p;
+    if (!is_inf(D) && D % 8 != 0) return {};
     // zero point: int8 everywhere; float8_e4m3fn (what the FP8 presets register) on the fp8 quantize / dequantize / fake_quantize kernels
     const bool fp8_op = (op == CT_OP_QUANTIZE && d.qtype == CT_Q_FLOAT) || (op == CT_OP_FAKE_QUANTIZE && d.qtype == CT_Q_FLOAT) ||
                         (op == CT_OP_DEQUANTIZE && d.q_dtype == CT_F8E4M3 && d.out_dtype == d.scale_dtype);
-    if (zp && d.zp_dtype != CT_I8 && !(d.zp_dtype == CT_F8E4M3 && fp8_op)) return p;
+    if (zp && d.zp_dtype != CT_I8 && !(d.zp_dtype == CT_F8E4M3 && fp8_op)) return {};
     const int zpk = zp ? (d.zp_dtype == CT_I8 ? 1 : 2) : 0;
+    // the largest thread unit (chunks) the layout admits: a unit must see one scale and must not straddle a row or the end of the tensor
+    int max_unit = 4;
+    while (max_unit > 1 && !((is_inf(D) || (D / 8) % max_unit == 0) && (!two_d || (d.cols / 8) % max_unit == 0) && (n / 8) % max_unit == 0))
+        max_unit /= 2;
 
     int p_dt, in_bytes_per_chunk;
-    FastSig sig;
-    sig.zp = zpk;
-    sig.group = 1;
+    StreamKernel k;
     switch (op) {
     case CT_OP_QUANTIZE_PACK:
-        if (d.qtype != CT_Q_INT || (d.num_bits != 4 && d.num_bits != 8)) return p;
-        if ((d.cols * d.num_bits) % 32 != 0) return p;
-        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || !is_float_dt(d.x_dtype)) return p;
-        p_dt = d.x_dtype; sig.op = F_QUANTPACK; sig.sel = d.num_bits; in_bytes_per_chunk = 8 * dt_size(p_dt);
-        sig.group = fast_group_quantpack(p_dt, d.num_bits);
+        if (d.qtype != CT_Q_INT || (d.num_bits != 4 && d.num_bits != 8)) return {};
+        if ((d.cols * d.num_bits) % 32 != 0) return {};
+        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || !is_float_dt(d.x_dtype)) return {};
+        p_dt = d.x_dtype; in_bytes_per_chunk = 8 * dt_size(p_dt);
+        k = quantpack_kernel(p_dt, d.num_bits, zpk, max_unit);
         break;
     case CT_OP_OBSERVE_QUANTIZE_PACK: {
         // fused observer: `scale` / `zp` are OUTPUTS; group strategy only, a group = 32 * {1,2,4,8} elements
-        if (d.qtype != CT_Q_INT || (d.num_bits != 4 && d.num_bits != 8)) return p;
-        if ((d.cols * d.num_bits) % 32 != 0 || n % 32 != 0) return p;
-        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16)) return p;
-        if (is_inf(D) || D != d.cdiv || D % 32 != 0) return p;
-        const int64_t lpg = D / 32;
-        if (lpg != 1 && lpg != 2 && lpg != 4 && lpg != 8) return p;
-        p_dt = d.x_dtype; sig.op = F_OBSERVE_QP; sig.sel = d.num_bits; in_bytes_per_chunk = 16;
-        sig.group = (int)lpg;
-        p.fast = true;
-        p.sig = sig;
-        p.sig.p_dt = p_dt;
-        p.job.in = reinterpret_cast<const uint8_t*>(in);
-        p.job.scale = scale;
-        p.job.zp = zp;
-        p.job.out = reinterpret_cast<uint8_t*>(out);
-        p.job.n_chunks = (uint32_t)(n / 8);
-        p.job.dc = make_fastdiv((uint64_t)(D / 8));
-        p.cm = make_common(p_dt, d.qtype, d.num_bits);
-        return p;
+        if (d.qtype != CT_Q_INT || (d.num_bits != 4 && d.num_bits != 8)) return {};
+        if ((d.cols * d.num_bits) % 32 != 0 || n % 32 != 0) return {};
+        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16)) return {};
+        if (is_inf(D) || D != d.cdiv || D % 32 != 0) return {};
+        p_dt = d.x_dtype; in_bytes_per_chunk = 16;
+        k = observe_kernel(p_dt, d.num_bits, zp != nullptr, (int)(D / 32));
+        break;
     }
     case CT_OP_UNPACK_DEQUANTIZE:
-        if (d.num_bits != 4 && d.num_bits != 8) return p;
-        if ((d.cols * d.num_bits) % 32 != 0) return p;
-        if (d.out_dtype != d.scale_dtype || !is_float_dt(d.out_dtype)) return p;
-        p_dt = d.scale_dtype; sig.op = F_UNPACKDEQ; sig.sel = d.num_bits; in_bytes_per_chunk = d.num_bits;
+        if (d.num_bits != 4 && d.num_bits != 8) return {};
+        if ((d.cols * d.num_bits) % 32 != 0) return {};
+        if (d.out_dtype != d.scale_dtype || !is_float_dt(d.out_dtype)) return {};
+        p_dt = d.scale_dtype; in_bytes_per_chunk = d.num_bits;
+        k = unpackdeq_kernel(p_dt, d.num_bits, zpk);
         break;
     case CT_OP_QUANTIZE:
-        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || !is_float_dt(d.x_dtype)) return p;
-        if (d.qtype == CT_Q_INT && d.q_dtype != CT_I8) return p;
-        if (d.qtype == CT_Q_FLOAT && d.q_dtype != CT_F8E4M3) return p;
-        p_dt = d.x_dtype; sig.op = F_QUANT; sig.sel = (d.qtype == CT_Q_FLOAT) ? 2 : 1; in_bytes_per_chunk = 8 * dt_size(p_dt);
-        sig.group = fast_group_quant(p_dt);
+        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || !is_float_dt(d.x_dtype)) return {};
+        if (d.qtype == CT_Q_INT && d.q_dtype != CT_I8) return {};
+        if (d.qtype == CT_Q_FLOAT && d.q_dtype != CT_F8E4M3) return {};
+        p_dt = d.x_dtype; in_bytes_per_chunk = 8 * dt_size(p_dt);
+        k = quant_kernel(p_dt, d.qtype == CT_Q_FLOAT, zpk, max_unit);
         break;
     case CT_OP_DEQUANTIZE:
         if (d.scale_dtype == CT_F32 && (d.out_dtype == CT_BF16 || d.out_dtype == CT_F16) && d.q_dtype == CT_F8E4M3 && !zp) {
-            // (q.to(float32) * scale).to(T): fp8 block checkpoints (DequantF32ScaleOp)
-            p_dt = d.out_dtype; sig.op = F_DEQUANT; sig.sel = 3; in_bytes_per_chunk = 8;
+            // (q.to(float32) * scale).to(T): fp8 block checkpoints
+            p_dt = d.out_dtype; in_bytes_per_chunk = 8;
+            k = dequant_kernel(p_dt, true, 0, true);
             break;
         }
-        if (d.out_dtype != d.scale_dtype || !is_float_dt(d.out_dtype)) return p;
-        if (d.q_dtype != CT_I8 && d.q_dtype != CT_F8E4M3) return p;
-        p_dt = d.scale_dtype; sig.op = F_DEQUANT; sig.sel = (d.q_dtype == CT_F8E4M3) ? 2 : 1; in_bytes_per_chunk = 8;
+        if (d.out_dtype != d.scale_dtype || !is_float_dt(d.out_dtype)) return {};
+        if (d.q_dtype != CT_I8 && d.q_dtype != CT_F8E4M3) return {};
+        p_dt = d.scale_dtype; in_bytes_per_chunk = 8;
+        k = dequant_kernel(p_dt, d.q_dtype == CT_F8E4M3, zpk, false);
         break;
     case CT_OP_FAKE_QUANTIZE:
-        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || d.out_dtype != d.x_dtype || !is_float_dt(d.x_dtype)) return p;
-        p_dt = d.x_dtype; sig.op = F_FAKE;
-        if (d.qtype == CT_Q_FLOAT) sig.sel = 2;
-        else sig.sel = (p_dt == CT_F32 || d.num_bits > (p_dt == CT_BF16 ? 7 : 8)) ? 1 : 0;
-        in_bytes_per_chunk = 8 * dt_size(p_dt);
+        if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || d.out_dtype != d.x_dtype || !is_float_dt(d.x_dtype)) return {};
+        p_dt = d.x_dtype; in_bytes_per_chunk = 8 * dt_size(p_dt);
+        k = fake_kernel(p_dt, d.qtype, d.num_bits, zpk);
         break;
     default:
-        return p;
-    }
-    sig.p_dt = p_dt;
-    // a thread unit (group of chunks) must see one scale and must not straddle the end of the tensor
-    if (sig.group > 1) {
-        const bool scale_ok = is_inf(D) || ((D / 8) % sig.group == 0);
-        const bool row_ok = !two_d || ((d.cols / 8) % sig.group == 0);
-        if (!scale_ok || !row_ok || (n / 8) % sig.group != 0) sig.group = 1;
+        return {};
     }
     // a partial last tile must still be a multiple of 16 bytes for the bulk copy
-    if (((n / 8) * in_bytes_per_chunk) % 16 != 0) return p;
-
-    p.fast = true;
-    p.sig = sig;
-    p.job.in = reinterpret_cast<const uint8_t*>(in);
-    p.job.scale = scale;
-    p.job.zp = zp;
-    p.job.out = reinterpret_cast<uint8_t*>(out);
-    p.job.n_chunks = (uint32_t)(n / 8);
-    p.job.dc = make_fastdiv(is_inf(D) ? (uint64_t)0x7FFFFFFFull : (uint64_t)(D / 8));
-    if (two_d) {
-        p.job.cpr = make_fastdiv((uint64_t)(d.cols / 8));
-        p.job.rd = make_fastdiv(is_inf(d.rdiv) ? (uint64_t)0x7FFFFFFFull : (uint64_t)d.rdiv);
-        p.job.srs = (uint32_t)d.s_row_stride;
-    }
-    p.cm = make_common(p_dt, d.qtype, d.num_bits);
-    return p;
+    if (((n / 8) * in_bytes_per_chunk) % 16 != 0) return {};
+    return fast_plan(k, make_common(p_dt, d.qtype, d.num_bits), in, scale, zp, out, nullptr, n, 8, D, two_d ? &d : nullptr);
 }
 
 // FP4 fused ops as streaming jobs (fast_fp4.cu).  Both need GROUP strategy with full rows of scales and no g_idx.
@@ -217,131 +194,60 @@ static Plan plan_one(int op, const ct_quant_desc& d, const void* in, const void*
 //   unpack+dequantize: out bf16 / fp16, units of 16 elements; scale in the out dtype or as stored (fp8 / E8M0)
 static Plan plan_fp4(int op, const ct_quant_desc& d, const void* in, const void* scale, const void* zp,
                      const int32_t* g_idx, void* out) {
-    Plan p;
-    p.fast = false;
-    memset(&p.job, 0, sizeof(p.job));
-    memset(&p.cm, 0, sizeof(p.cm));
-    p.sig = FastSig{0, 0, 0, 0, 1};
     const int64_t n = d.rows * d.cols;
     int64_t D;
-    if (g_idx || n == 0 || (n / 8) >= 0x7fffffffLL || !aligned16(in) || !aligned16(out)) return p;
-    if (!flat_divisor(d, D) || is_inf(D) || d.qtype != CT_Q_FP4) return p;
-    FastSig sig{0, 0, 0, 0, 1};
+    if (g_idx || n == 0 || (n / 8) >= 0x7fffffffLL || !aligned16(in) || !aligned16(out)) return {};
+    if (!flat_divisor(d, D) || is_inf(D) || d.qtype != CT_Q_FP4) return {};
+    StreamKernel k;
+    int p_dt;
     if (op == CT_OP_OBSERVE_QUANTIZE_PACK_FP4) {
         // scale (float8_e4m3fn [rows, cols / 16]) is an OUTPUT; NVFP4 only: group 16, float32 global scale given, no zero point
-        if ((d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) || d.cols % 32 != 0 || D != 16 || !d.global_scale || zp) return p;
-        if ((reinterpret_cast<uintptr_t>(scale) & 1u) != 0) return p;
-        sig.op = F_FP4_QUANTPACK; sig.p_dt = d.x_dtype; sig.group = 4; sig.sel = 3;
+        if ((d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) || d.cols % 32 != 0 || D != 16 || !d.global_scale || zp) return {};
+        if ((reinterpret_cast<uintptr_t>(scale) & 1u) != 0) return {};
+        p_dt = d.x_dtype;
+        k = fp4_observe_kernel(p_dt);
     } else if (op == CT_OP_QUANTIZE_PACK_FP4) {
-        if (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) return p;
-        if (d.cols % 32 != 0 || !aligned16(scale) ) return p;
-        sig.op = F_FP4_QUANTPACK; sig.p_dt = d.x_dtype; sig.group = 4;
-        if (d.global_scale) {
-            if (D != 16 || d.seff_dtype != CT_F32 || d.compute_dtype != CT_F32) return p;
-            if (d.scale_dtype == d.x_dtype) sig.sel = 1;
-            else if (d.scale_dtype == CT_F32) sig.sel = 2;
-            else return p;
-            if (zp) { if (d.zp_dtype != CT_F8E4M3) return p; sig.zp = 1; }   // FZ_F8
-        } else {
-            if (D % 32 != 0 || d.scale_dtype != d.x_dtype || d.compute_dtype != d.x_dtype) return p;
-            sig.sel = 0;
-            if (zp) {
-                if (d.zp_dtype == CT_U8) sig.zp = 2;        // FZ_U8
-                else if (d.zp_dtype == CT_I8) sig.zp = 3;   // FZ_I8
-                else return p;
-            }
-        }
+        if (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) return {};
+        if (d.cols % 32 != 0 || !aligned16(scale) ) return {};
+        if (d.global_scale ? (D != 16 || d.seff_dtype != CT_F32 || d.compute_dtype != CT_F32) : (D % 32 != 0 || d.compute_dtype != d.x_dtype)) return {};
+        p_dt = d.x_dtype;
+        k = fp4_quantpack_kernel(p_dt, d.global_scale != nullptr, d.scale_dtype, zp ? d.zp_dtype : CT_NONE);
     } else {
-        if (d.out_dtype != CT_BF16 && d.out_dtype != CT_F16) return p;
-        if (zp || d.cols % 8 != 0 || D % 8 != 0) return p;
-        sig.op = F_FP4_UNPACKDEQ; sig.p_dt = d.out_dtype; sig.group = 1;
-        if (d.scale_dtype == d.out_dtype) sig.sel = 0;          // FS_SAME
-        else if (d.scale_dtype == CT_F8E4M3) sig.sel = 2;       // FS_F8
-        else if (d.scale_dtype == CT_E8M0) sig.sel = 3;         // FS_E8M0
-        else return p;
-        if (d.global_scale ? d.seff_dtype != CT_F32 : (d.seff_dtype != d.out_dtype && d.scale_dtype != d.out_dtype)) return p;
-        if (((n / 8) * 4) % 16 != 0) return p;   // a partial last tile must still be a multiple of 16 bytes for the bulk copy
+        if (d.out_dtype != CT_BF16 && d.out_dtype != CT_F16) return {};
+        if (zp || d.cols % 8 != 0 || D % 8 != 0) return {};
+        if (d.global_scale ? d.seff_dtype != CT_F32 : (d.seff_dtype != d.out_dtype && d.scale_dtype != d.out_dtype)) return {};
+        if (((n / 8) * 4) % 16 != 0) return {};   // a partial last tile must still be a multiple of 16 bytes for the bulk copy
+        p_dt = d.out_dtype;
+        k = fp4_unpackdeq_kernel(p_dt, d.scale_dtype);
     }
-    p.fast = true;
-    p.sig = sig;
-    p.job.in = reinterpret_cast<const uint8_t*>(in);
-    p.job.scale = scale;
-    p.job.zp = zp;
-    p.job.out = reinterpret_cast<uint8_t*>(out);
-    p.job.aux = d.global_scale;
-    p.job.n_chunks = (uint32_t)(n / 8);
-    p.job.dc = make_fastdiv((uint64_t)(D / 8));
-    p.cm = make_common(sig.p_dt, CT_Q_FP4, 4);
-    return p;
+    return fast_plan(k, make_common(p_dt, CT_Q_FP4, 4), in, scale, zp, out, d.global_scale, n, 8, D);
 }
 
 // fused 2:4 select + int4 (fast_sparse24q.cu).  compress: chunk = 8 dense elements, unit = 4 chunks; decompress: chunk = 16 dense
 // elements (4 bytes of nibbles) = one unit.  Full rows of scales only (flat scale index), cols % 32 == 0.
 static Plan plan_s24(int op, const ct_quant_desc& d, const void* in, const void* scale, const void* zp, const int32_t* g_idx, void* out) {
-    Plan p;
-    p.fast = false;
-    memset(&p.job, 0, sizeof(p.job));
-    memset(&p.cm, 0, sizeof(p.cm));
-    p.sig = FastSig{0, 0, 0, 0, 1};
     const int64_t n = d.rows * d.cols;
     int64_t D;
-    if (g_idx || n == 0 || n % 64 != 0 || d.cols % 32 != 0 || (n / 8) >= 0x7fffffffLL || !aligned16(in) || !aligned16(out)) return p;
-    if (!d.aux || (reinterpret_cast<uintptr_t>(d.aux) & 3u) != 0 || d.global_scale || d.qtype != CT_Q_INT || d.num_bits != 4) return p;
-    if (!flat_divisor(d, D) || (!is_inf(D) && D % 32 != 0)) return p;
-    if (zp && d.zp_dtype != CT_I8) return p;
+    if (g_idx || n == 0 || n % 64 != 0 || d.cols % 32 != 0 || (n / 8) >= 0x7fffffffLL || !aligned16(in) || !aligned16(out)) return {};
+    if (!d.aux || (reinterpret_cast<uintptr_t>(d.aux) & 3u) != 0 || d.global_scale || d.qtype != CT_Q_INT || d.num_bits != 4) return {};
+    if (!flat_divisor(d, D) || (!is_inf(D) && D % 32 != 0)) return {};
+    if (zp && d.zp_dtype != CT_I8) return {};
     const bool comp = (op == CT_OP_SPARSE24_QUANTIZE_PACK);
-    if (!comp && (reinterpret_cast<uintptr_t>(out) & 31u) != 0) return p;   // the expansion writes with 256-bit stores
+    if (!comp && (reinterpret_cast<uintptr_t>(out) & 31u) != 0) return {};   // the expansion writes with 256-bit stores
     const int p_dt = comp ? d.x_dtype : d.out_dtype;
-    if (p_dt != CT_BF16 && p_dt != CT_F16) return p;
-    if (d.scale_dtype != p_dt || (comp && d.compute_dtype != p_dt)) return p;
-    const int64_t chunk = comp ? 8 : 16;
-    p.fast = true;
-    p.sig = FastSig{comp ? F_S24_QUANTPACK : F_S24_UNPACKDEQ, p_dt, 4, zp ? 1 : 0, comp ? 4 : 1};
-    p.job.in = reinterpret_cast<const uint8_t*>(in);
-    p.job.scale = scale;
-    p.job.zp = zp;
-    p.job.out = reinterpret_cast<uint8_t*>(out);
-    p.job.aux = d.aux;
-    p.job.n_chunks = (uint32_t)(n / chunk);
-    p.job.dc = make_fastdiv(is_inf(D) ? (uint64_t)0x7FFFFFFFull : (uint64_t)(D / chunk));
-    p.cm = make_common(p_dt, CT_Q_INT, 4);
-    return p;
+    if (p_dt != CT_BF16 && p_dt != CT_F16) return {};
+    if (d.scale_dtype != p_dt || (comp && d.compute_dtype != p_dt)) return {};
+    return fast_plan(sparse24q_kernel(comp, p_dt, zp ? 1 : 0), make_common(p_dt, CT_Q_INT, 4), in, scale, zp, out, d.aux, n, comp ? 8 : 16, D);
 }
 
 // standalone pack / unpack (packed_dim 1) as a streaming job; for these ops a chunk is 16 codes
 static Plan plan_bits(bool pack, int64_t rows, int64_t cols, int bits, const void* in, void* out) {
-    Plan p;
-    p.fast = false;
-    memset(&p.job, 0, sizeof(p.job));
-    p.cm = make_common(CT_F32, CT_Q_INT, bits);
-    p.sig = FastSig{pack ? F_PACK : F_UNPACK, CT_I8, bits, 0, 1};
     const int64_t n = rows * cols;
     const int in_bytes = pack ? 16 : 2 * bits;
     const int unit = (pack && bits == 4) ? 32 : 16;   // 4-bit packing works on units of 2 chunks
-    if (!(bits == 4 || bits == 8) || (cols * bits) % 32 != 0 || n == 0 || n % unit != 0 || (n / 16) >= 0x7fffffffLL) return p;
-    if (!aligned16(in) || !aligned16(out) || ((n / 16) * in_bytes) % 16 != 0) return p;
-    p.fast = true;
-    p.job.in = reinterpret_cast<const uint8_t*>(in);
-    p.job.out = reinterpret_cast<uint8_t*>(out);
-    p.job.n_chunks = (uint32_t)(n / 16);
-    p.job.dc = make_fastdiv(0x7FFFFFFFull);
-    return p;
-}
-
-static int launch_sig(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.op) {
-    case F_QUANTPACK: return launch_fast_quantpack(s, lp, device, st);
-    case F_UNPACKDEQ: return launch_fast_unpackdeq(s, lp, device, st);
-    case F_QUANT: return launch_fast_quant(s, lp, device, st);
-    case F_DEQUANT: return launch_fast_dequant(s, lp, device, st);
-    case F_FAKE: return launch_fast_fake(s, lp, device, st);
-    case F_OBSERVE_QP: return launch_fast_observe(s, lp, device, st);
-    case F_FP4_QUANTPACK:
-    case F_FP4_UNPACKDEQ: return launch_fast_fp4(s, lp, device, st);
-    case F_S24_QUANTPACK:
-    case F_S24_UNPACKDEQ: return launch_fast_sparse24q(s, lp, device, st);
-    default: return launch_fast_bits(s, lp, device, st);
-    }
+    if (!(bits == 4 || bits == 8) || (cols * bits) % 32 != 0 || n == 0 || n % unit != 0 || (n / 16) >= 0x7fffffffLL) return {};
+    if (!aligned16(in) || !aligned16(out) || ((n / 16) * in_bytes) % 16 != 0) return {};
+    return fast_plan(bits_kernel(pack, bits), make_common(CT_F32, CT_Q_INT, bits), in, nullptr, nullptr, out, nullptr, n, 16, CT_DIV_INF);
 }
 
 static int run_generic(int op, const ct_quant_desc& d, const void* in, const void* scale, const void* zp,
@@ -451,11 +357,11 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
         else if (op == CT_OP_SPARSE24_QUANTIZE_PACK || op == CT_OP_SPARSE24_UNPACK_DEQUANTIZE) plans[i] = plan_s24(op, descs[i], in[i], scale[i], z, g_idx ? g_idx[i] : nullptr, out[i]);
         else plans[i] = plan_one(op, descs[i], in[i], scale[i], z, g_idx ? g_idx[i] : nullptr, out[i]);
     }
-    // group fast jobs by kernel signature (and clamp constants), one launch per group
+    // group fast jobs by kernel (and clamp constants), one launch per group
     std::vector<char> done((size_t)n, 0);
     for (int i = 0; i < n; ++i) {
         if (done[i]) continue;
-        if (!plans[i].fast) {
+        if (!plans[i].k.launch) {
             // an empty tensor has nothing to compute, whatever op it is in (the fused-only ops would otherwise refuse it)
             if (descs[i].rows * descs[i].cols == 0) { done[i] = 1; continue; }
             if (bits_op) {
@@ -473,9 +379,10 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
         }
         std::vector<Job> jobs;
         uint32_t tiles = 0;
-        const uint32_t tc = (uint32_t)sig_tile_chunks(plans[i].sig);
+        const StreamKernel kern = plans[i].k;
+        const uint32_t tc = (uint32_t)kern.tile_chunks;
         for (int k = i; k < n; ++k) {
-            if (done[k] || !plans[k].fast || !(plans[k].sig == plans[i].sig) || plans[k].cm.bits != plans[i].cm.bits) continue;
+            if (done[k] || plans[k].k.launch != kern.launch || plans[k].cm.bits != plans[i].cm.bits) continue;
             const uint32_t nt = (plans[k].job.n_chunks + tc - 1) / tc;
             if ((uint64_t)tiles + nt >= 0xffffffffull) break;
             Job j = plans[k].job;
@@ -488,7 +395,6 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
         LaunchPlan lp;
         lp.cm = plans[i].cm;
         lp.total_tiles = tiles;
-        lp.tile_chunks = (int)tc;
         lp.tbl.n = (int)jobs.size();
         lp.tbl.jobs = nullptr;
         lp.tbl.one = jobs[0];
@@ -502,30 +408,16 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
             const size_t tbl_bytes = many ? jobs.size() * sizeof(Job) : 0;
             rc = scratch_alloc(reinterpret_cast<void**>(&scratch), 16 + tbl_bytes, device, stream);
             if (rc) return rc;
-            cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
-            if (many) cudaStreamIsCapturing(stream, &capturing);
-            if (many && capturing == cudaStreamCaptureStatusActive) {
-                CT_CUDA_TRY(cudaMemsetAsync(scratch, 0, 16, stream));
-                for (size_t o = 0; o < jobs.size(); o += 32) {
-                    JobBlock blk;
-                    const int cnt = (int)(jobs.size() - o < 32 ? jobs.size() - o : 32);
-                    memcpy(blk.j, jobs.data() + o, (size_t)cnt * sizeof(Job));
-                    upload_jobs_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<Job*>(scratch + 16) + o, blk, cnt);
-                }
-                count_launch((int)((jobs.size() + 31) / 32));
-                CT_CUDA_TRY(cudaGetLastError());
-                lp.tbl.jobs = reinterpret_cast<const Job*>(scratch + 16);
-            } else if (many) {
-                std::vector<uint8_t> img(16 + tbl_bytes, 0);
-                memcpy(img.data() + 16, jobs.data(), tbl_bytes);
-                CT_CUDA_TRY(cudaMemcpyAsync(scratch, img.data(), img.size(), cudaMemcpyHostToDevice, stream));
+            if (many) {
+                rc = upload_jobs<Job, 32>(scratch, 16, jobs.data(), jobs.size(), stream);   // 32 jobs = 3.3 KB of kernel parameters
+                if (rc) return rc;
                 lp.tbl.jobs = reinterpret_cast<const Job*>(scratch + 16);
             } else {
                 CT_CUDA_TRY(cudaMemsetAsync(scratch, 0, 16, stream));
             }
             if (dynamic) lp.sched = reinterpret_cast<uint32_t*>(scratch);
         }
-        rc = launch_sig(plans[i].sig, lp, device, stream);
+        rc = kern.launch(lp, device, stream);
         if (scratch) cudaFreeAsync(scratch, stream);
         if (rc) return rc;
     }
@@ -550,33 +442,22 @@ static int run_bits(bool pack, const void* in, void* out, int64_t rows, int64_t 
     if (packed_dim != 0 && packed_dim != 1) { set_error("packed_dim must be 0 or 1"); return CT_E_ARG; }
     if (rows < 0 || cols < 0) { set_error("negative shape"); return CT_E_SHAPE; }
     if (device == CT_DEVICE_CPU) return cpu_run_bits(pack, in, out, rows, cols, bits, packed_dim);
+    if (packed_dim == 1) {   // as one tensor of ct_batched: the streaming kernel where the layout admits it, the generic one otherwise
+        ct_quant_desc d;
+        memset(&d, 0, sizeof(d));
+        d.rows = rows;
+        d.cols = cols;
+        d.num_bits = bits;
+        const void* ins[1] = {in};
+        void* outs[1] = {out};
+        return run_batched(pack ? CT_OP_PACK_INT32 : CT_OP_UNPACK_INT32, 1, &d, ins, nullptr, nullptr, nullptr, outs, device, stream);
+    }
     int rc = check_device(device);
     if (rc) return rc;
     if (rows * cols == 0) return CT_OK;
     if (!in || !out) { set_error("null tensor pointer"); return CT_E_ARG; }
     DeviceGuard guard(device);
     if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice");
-    const int64_t n = rows * cols;
-    // for these two ops a chunk is 16 codes; 4-bit packing works on units of 2 chunks
-    const int in_bytes = pack ? 16 : 2 * bits;
-    const int unit = (pack && bits == 4) ? 32 : 16;
-    if (packed_dim == 1 && (bits == 4 || bits == 8) && (cols * bits) % 32 == 0 && n % unit == 0 && (n / 16) < 0x7fffffffLL &&
-        aligned16(in) && aligned16(out) && ((n / 16) * in_bytes) % 16 == 0) {
-        LaunchPlan lp;
-        memset(&lp, 0, sizeof(lp));
-        lp.tbl.n = 1;
-        lp.tbl.one.in = reinterpret_cast<const uint8_t*>(in);
-        lp.tbl.one.out = reinterpret_cast<uint8_t*>(out);
-        lp.tbl.one.n_chunks = (uint32_t)(n / 16);
-        lp.tbl.one.tile_begin = 0;
-        lp.tbl.one.tile_end = (lp.tbl.one.n_chunks + TILE_CHUNKS - 1) / TILE_CHUNKS;
-        lp.tbl.one.dc = make_fastdiv(0x7FFFFFFFull);
-        lp.total_tiles = lp.tbl.one.tile_end;
-        lp.tile_chunks = TILE_CHUNKS;
-        lp.cm = make_common(CT_F32, CT_Q_INT, bits);
-        FastSig s{pack ? F_PACK : F_UNPACK, CT_I8, bits, 0, 1};
-        return launch_fast_bits(s, lp, device, stream);
-    }
     if (pack) return launch_generic_pack(reinterpret_cast<const int8_t*>(in), reinterpret_cast<int32_t*>(out), rows, cols, bits, packed_dim, stream);
     return launch_generic_unpack(reinterpret_cast<const int32_t*>(in), reinterpret_cast<int8_t*>(out), rows, cols, bits, packed_dim, stream);
 }

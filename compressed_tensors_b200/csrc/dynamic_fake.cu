@@ -236,9 +236,9 @@ extern "C" int ct_dynamic_fake_quantize(const ct_quant_desc* d, int asymmetric, 
     if (!gs && d->scale_dtype != xdt) return unsupported("the scale is held in x's dtype without a global scale");
     if (n == 0) return CT_OK;
     if (!x || !out || !scale_out || !zp_out) { set_error("null tensor pointer"); return CT_E_ARG; }
-    // the element rule ct_fake_quantize takes for the same tensors (dispatch.cu, plan_one)
+    // the element rule ct_fake_quantize takes for the same tensors
     const bool fast = !gs && !fp4_q && d->compute_dtype == xdt && d->seff_dtype == xdt && (d->zp_dtype == CT_I8 || (d->zp_dtype == CT_F8E4M3 && fp8_q));
-    const int kind = !fast ? K_SCALAR : fp8_q ? QF8 : (d->num_bits > (xdt == CT_BF16 ? 7 : 8) ? QI_WIDE : QI_NARROW);
+    const int kind = fast ? fake_kind(xdt, d->qtype, d->num_bits) : K_SCALAR;
 
     const bool tensor = is_inf_div(d->rdiv) && is_inf_div(d->cdiv);
     const bool token = d->rdiv == 1 && d->s_row_stride == 1 && is_inf_div(d->cdiv);

@@ -6,38 +6,20 @@
 
 namespace ctb {
 
-// ---- fast (flat, streaming) path -------------------------------------------------------
-enum FastOp { F_QUANTPACK = 0, F_UNPACKDEQ = 1, F_QUANT = 2, F_DEQUANT = 3, F_FAKE = 4, F_PACK = 5, F_UNPACK = 6, F_OBSERVE_QP = 7,
-              F_FP4_QUANTPACK = 8, F_FP4_UNPACKDEQ = 9, F_S24_QUANTPACK = 10, F_S24_UNPACKDEQ = 11 };
-
-struct FastSig {
-    int op;      // FastOp
-    int p_dt;    // CT_BF16 / CT_F16 / CT_F32 (unused for F_PACK / F_UNPACK)
-    int sel;     // QUANTPACK/UNPACKDEQ/PACK/UNPACK: bits (4 | 8); QUANT/DEQUANT/FAKE: QKind
-    int zp;      // 0 none, 1 int8, 2 float8_e4m3fn (fp8 quantize / dequantize / fake_quantize only)
-    int group;   // chunks per thread unit (1, 2 or 4): stream.cuh
-    bool operator==(const FastSig& o) const { return op == o.op && p_dt == o.p_dt && sel == o.sel && zp == o.zp && group == o.group; }
-};
-
-// chunks per tile of the kernel a signature selects (stream.cuh: TileOf<Op>): the 16-bit quantize+pack, unpack+dequantize, quantize and
-// dequantize functors run on the big tile
-static inline int sig_tile_chunks(const FastSig& s) {
-    const bool p16 = (s.p_dt == CT_BF16 || s.p_dt == CT_F16);
-    return (p16 && (s.op == F_QUANTPACK || s.op == F_UNPACKDEQ || s.op == F_QUANT || s.op == F_DEQUANT)) ? BIG_TILE_CHUNKS : TILE_CHUNKS;
-}
-
-// defined in fast_pack.cu / fast_quant.cu / fast_fake.cu
-int launch_fast_quantpack(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int launch_fast_unpackdeq(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int launch_fast_quant(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int launch_fast_dequant(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int launch_fast_fake(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int launch_fast_bits(const FastSig&, const LaunchPlan&, int device, cudaStream_t);
-int fast_group_quantpack(int p_dt, int bits);   // preferred unit size of the instantiated kernels
-int fast_group_quant(int p_dt);
-int launch_fast_fp4(const FastSig&, const LaunchPlan&, int device, cudaStream_t);       // fast_fp4.cu; sig.sel / sig.zp: see there
-int launch_fast_observe(const FastSig&, const LaunchPlan&, int device, cudaStream_t);   // fast_observe.cu; sig.group = lanes per quantization group
-int launch_fast_sparse24q(const FastSig&, const LaunchPlan&, int device, cudaStream_t); // fast_sparse24q.cu: fused 2:4 select + int4 (BASELINE config 4)
+// ---- fast (flat, streaming) path: one selector per kernel family, defined in the file that instantiates it -----------------
+// Each returns the kernel for its arguments, or one with a null `launch` when no instantiation exists.  p_dt: CT_BF16 / CT_F16 / CT_F32;
+// zp_kind: 0 none, 1 int8, 2 float8_e4m3fn; max_unit: the largest thread unit (chunks; 4, 2 or 1) the tensor's layout admits.
+StreamKernel quantpack_kernel(int p_dt, int bits, int zp_kind, int max_unit);   // fast_pack.cu
+StreamKernel unpackdeq_kernel(int p_dt, int bits, int zp_kind);
+StreamKernel bits_kernel(bool pack, int bits);                                  // standalone int8 <-> int32 packing
+StreamKernel quant_kernel(int p_dt, bool fp8, int zp_kind, int max_unit);       // fast_quant.cu
+StreamKernel dequant_kernel(int p_dt, bool fp8, int zp_kind, bool f32_scale);   // f32_scale: fp8 codes, float32 scale, 16-bit output
+StreamKernel fake_kernel(int p_dt, int qtype, int bits, int zp_kind);           // fast_fake.cu
+StreamKernel observe_kernel(int p_dt, int bits, bool asym, int lanes_per_group); // fast_observe.cu
+StreamKernel fp4_quantpack_kernel(int p_dt, bool global_scale, int scale_dt, int zp_dt);   // fast_fp4.cu; zp_dt CT_NONE: no zero point
+StreamKernel fp4_observe_kernel(int p_dt);
+StreamKernel fp4_unpackdeq_kernel(int p_dt, int scale_dt);
+StreamKernel sparse24q_kernel(bool compress, int p_dt, int zp_kind);            // fast_sparse24q.cu: fused 2:4 select + int4
 
 // ---- generic path (any strategy, g_idx, ragged shapes, mixed dtypes) -----------------------
 enum GenericMode { G_QUANTIZE = 0, G_DEQUANTIZE = 1, G_FAKE = 2 };

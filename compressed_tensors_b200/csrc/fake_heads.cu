@@ -162,8 +162,7 @@ extern "C" int ct_fake_quantize_heads(int n, const ct_head_job* jobs, int device
     if (total == 0) return CT_OK;
     const int p_dt = j0.x_dtype;
     L.cm = make_common(p_dt, j0.qtype, j0.num_bits);
-    // the rounding kind ct_fake_quantize picks for the same problem (dispatch.cu, plan_one)
-    const int kind = (j0.qtype == CT_Q_FLOAT) ? QF8 : ((p_dt == CT_F32 || j0.num_bits > (p_dt == CT_BF16 ? 7 : 8)) ? QI_WIDE : QI_NARROW);
+    const int kind = fake_kind(p_dt, j0.qtype, j0.num_bits);
     const int zpk = zp_kind(j0);
     DeviceGuard guard(device);
     if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice");

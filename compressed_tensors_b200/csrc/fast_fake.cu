@@ -4,41 +4,28 @@
 
 namespace ctb {
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fast kernel for op=%d dtype=%d sel=%d zp=%d group=%d", sig.op, sig.p_dt, sig.sel, sig.zp, sig.group); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
 template <class P>
-static int fake_by(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == QF8 && s.zp == 0) return launch_stream<FakeQuantOp<P, QF8, 0>>(lp, device, st);
-    if (s.sel == QF8 && s.zp == 1) return launch_stream<FakeQuantOp<P, QF8, 1>>(lp, device, st);
-    if (s.sel == QF8 && s.zp == 2) return launch_stream<FakeQuantOp<P, QF8, 2>>(lp, device, st);
-    if (s.sel == QI_NARROW && s.zp == 0) return launch_stream<FakeQuantOp<P, QI_NARROW, 0>>(lp, device, st);
-    if (s.sel == QI_NARROW && s.zp == 1) return launch_stream<FakeQuantOp<P, QI_NARROW, 1>>(lp, device, st);
-    if (s.sel == QI_WIDE && s.zp == 0) return launch_stream<FakeQuantOp<P, QI_WIDE, 0>>(lp, device, st);
-    if (s.sel == QI_WIDE && s.zp == 1) return launch_stream<FakeQuantOp<P, QI_WIDE, 1>>(lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel fake_p(int kind, int zp_kind) {
+    if (kind == QF8 && zp_kind == 0) return stream_kernel<FakeQuantOp<P, QF8, 0>>();
+    if (kind == QF8 && zp_kind == 1) return stream_kernel<FakeQuantOp<P, QF8, 1>>();
+    if (kind == QF8 && zp_kind == 2) return stream_kernel<FakeQuantOp<P, QF8, 2>>();
+    if (kind == QI_WIDE && zp_kind == 0) return stream_kernel<FakeQuantOp<P, QI_WIDE, 0>>();
+    if (kind == QI_WIDE && zp_kind == 1) return stream_kernel<FakeQuantOp<P, QI_WIDE, 1>>();
+    if constexpr (P::DT != CT_F32) {   // fp32 has no packed-magic rounding: fake_kind never picks NARROW for it
+        if (kind == QI_NARROW && zp_kind == 0) return stream_kernel<FakeQuantOp<P, QI_NARROW, 0>>();
+        if (kind == QI_NARROW && zp_kind == 1) return stream_kernel<FakeQuantOp<P, QI_NARROW, 1>>();
+    }
+    return {};
 }
 
-int launch_fast_fake(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.p_dt) {
-    case CT_BF16: return fake_by<BF16>(s, lp, device, st);
-    case CT_F16: return fake_by<F16>(s, lp, device, st);
-    case CT_F32: {
-        // fp32 has no packed-magic rounding: NARROW and WIDE coincide
-        FastSig t = s;
-        if (t.sel == QI_NARROW) t.sel = QI_WIDE;
-        if (t.sel == QF8 && t.zp == 0) return launch_stream<FakeQuantOp<F32, QF8, 0>>(lp, device, st);
-        if (t.sel == QF8 && t.zp == 1) return launch_stream<FakeQuantOp<F32, QF8, 1>>(lp, device, st);
-        if (t.sel == QF8 && t.zp == 2) return launch_stream<FakeQuantOp<F32, QF8, 2>>(lp, device, st);
-        if (t.sel == QI_WIDE && t.zp == 0) return launch_stream<FakeQuantOp<F32, QI_WIDE, 0>>(lp, device, st);
-        if (t.sel == QI_WIDE && t.zp == 1) return launch_stream<FakeQuantOp<F32, QI_WIDE, 1>>(lp, device, st);
-        SIG_FAIL(s);
+StreamKernel fake_kernel(int p_dt, int qtype, int bits, int zp_kind) {
+    const int kind = fake_kind(p_dt, qtype, bits);
+    switch (p_dt) {
+    case CT_BF16: return fake_p<BF16>(kind, zp_kind);
+    case CT_F16: return fake_p<F16>(kind, zp_kind);
+    case CT_F32: return fake_p<F32>(kind, zp_kind);
     }
-    }
-    SIG_FAIL(s);
+    return {};
 }
 
 }  // namespace ctb

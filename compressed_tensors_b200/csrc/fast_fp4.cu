@@ -5,53 +5,49 @@
 
 namespace ctb {
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fast fp4 kernel for op=%d dtype=%d sel=%d zp=%d", sig.op, sig.p_dt, sig.sel, sig.zp); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
-// sig.sel: F_FP4_QUANTPACK: 0 = MX (arithmetic in T), 1 = NV with scale in T, 2 = NV with float32 scale, 3 = NV with the group
-//          observer fused in (scale is an OUTPUT, float8_e4m3fn)
-//          F_FP4_UNPACKDEQ: Fp4ScaleKind of the scale tensor (FS_SAME / FS_F8 / FS_E8M0)
-// sig.zp : Fp4ZpKind
+// quantize + pack.  Without a global scale: MX-style, scale and arithmetic in T, zero point absent, uint8 or int8.  With one: NVFP4,
+// float32 arithmetic, scale in T or float32, zero point absent or float8_e4m3fn.
 template <class P>
-static int fp4_quantpack_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == 0) {
-        if (s.zp == FZ_NONE) return launch_stream<Fp4MxQuantPackOp<P, FZ_NONE>>(lp, device, st);
-        if (s.zp == FZ_U8) return launch_stream<Fp4MxQuantPackOp<P, FZ_U8>>(lp, device, st);
-        if (s.zp == FZ_I8) return launch_stream<Fp4MxQuantPackOp<P, FZ_I8>>(lp, device, st);
-    } else if (s.sel == 1) {
-        if (s.zp == FZ_NONE) return launch_stream<Fp4NvQuantPackOp<P, FS_SAME, FZ_NONE>>(lp, device, st);
-        if (s.zp == FZ_F8) return launch_stream<Fp4NvQuantPackOp<P, FS_SAME, FZ_F8>>(lp, device, st);
-    } else if (s.sel == 2) {
-        if (s.zp == FZ_NONE) return launch_stream<Fp4NvQuantPackOp<P, FS_F32, FZ_NONE>>(lp, device, st);
-        if (s.zp == FZ_F8) return launch_stream<Fp4NvQuantPackOp<P, FS_F32, FZ_F8>>(lp, device, st);
+static StreamKernel fp4_quantpack_p(bool global_scale, int scale_dt, int zp_dt) {
+    if (!global_scale) {
+        if (scale_dt != P::DT) return {};
+        if (zp_dt == CT_NONE) return stream_kernel<Fp4MxQuantPackOp<P, FZ_NONE>>();
+        if (zp_dt == CT_U8) return stream_kernel<Fp4MxQuantPackOp<P, FZ_U8>>();
+        if (zp_dt == CT_I8) return stream_kernel<Fp4MxQuantPackOp<P, FZ_I8>>();
+    } else if (scale_dt == P::DT) {
+        if (zp_dt == CT_NONE) return stream_kernel<Fp4NvQuantPackOp<P, FS_SAME, FZ_NONE>>();
+        if (zp_dt == CT_F8E4M3) return stream_kernel<Fp4NvQuantPackOp<P, FS_SAME, FZ_F8>>();
+    } else if (scale_dt == CT_F32) {
+        if (zp_dt == CT_NONE) return stream_kernel<Fp4NvQuantPackOp<P, FS_F32, FZ_NONE>>();
+        if (zp_dt == CT_F8E4M3) return stream_kernel<Fp4NvQuantPackOp<P, FS_F32, FZ_F8>>();
     }
-    SIG_FAIL(s);
+    return {};
 }
-template <class P>
-static int fp4_unpackdeq_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == FS_SAME) return launch_stream<Fp4UnpackDequantOp<P, FS_SAME>>(lp, device, st);
-    if (s.sel == FS_F8) return launch_stream<Fp4UnpackDequantOp<P, FS_F8>>(lp, device, st);
-    if (s.sel == FS_E8M0) return launch_stream<Fp4UnpackDequantOp<P, FS_E8M0>>(lp, device, st);
-    SIG_FAIL(s);
+StreamKernel fp4_quantpack_kernel(int p_dt, bool global_scale, int scale_dt, int zp_dt) {
+    if (p_dt == CT_BF16) return fp4_quantpack_p<BF16>(global_scale, scale_dt, zp_dt);
+    if (p_dt == CT_F16) return fp4_quantpack_p<F16>(global_scale, scale_dt, zp_dt);
+    return {};
 }
 
-int launch_fast_fp4(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.op == F_FP4_QUANTPACK && s.sel == 3) {   // observe + quantize + pack (scale is an output)
-        if (s.p_dt == CT_BF16) return launch_stream<Fp4NvObserveQuantPackOp<BF16>>(lp, device, st);
-        if (s.p_dt == CT_F16) return launch_stream<Fp4NvObserveQuantPackOp<F16>>(lp, device, st);
-        SIG_FAIL(s);
-    }
-    if (s.op == F_FP4_QUANTPACK) {
-        if (s.p_dt == CT_BF16) return fp4_quantpack_p<BF16>(s, lp, device, st);
-        if (s.p_dt == CT_F16) return fp4_quantpack_p<F16>(s, lp, device, st);
-    } else {
-        if (s.p_dt == CT_BF16) return fp4_unpackdeq_p<BF16>(s, lp, device, st);
-        if (s.p_dt == CT_F16) return fp4_unpackdeq_p<F16>(s, lp, device, st);
-    }
-    SIG_FAIL(s);
+// NVFP4 observe + quantize + pack: the float8_e4m3fn scale is an OUTPUT
+StreamKernel fp4_observe_kernel(int p_dt) {
+    if (p_dt == CT_BF16) return stream_kernel<Fp4NvObserveQuantPackOp<BF16>>();
+    if (p_dt == CT_F16) return stream_kernel<Fp4NvObserveQuantPackOp<F16>>();
+    return {};
+}
+
+// unpack + dequantize: the scale in the output dtype, or as stored (float8_e4m3fn / E8M0)
+template <class P>
+static StreamKernel fp4_unpackdeq_p(int scale_dt) {
+    if (scale_dt == P::DT) return stream_kernel<Fp4UnpackDequantOp<P, FS_SAME>>();
+    if (scale_dt == CT_F8E4M3) return stream_kernel<Fp4UnpackDequantOp<P, FS_F8>>();
+    if (scale_dt == CT_E8M0) return stream_kernel<Fp4UnpackDequantOp<P, FS_E8M0>>();
+    return {};
+}
+StreamKernel fp4_unpackdeq_kernel(int p_dt, int scale_dt) {
+    if (p_dt == CT_BF16) return fp4_unpackdeq_p<BF16>(scale_dt);
+    if (p_dt == CT_F16) return fp4_unpackdeq_p<F16>(scale_dt);
+    return {};
 }
 
 // ---- selftest: the E2M1 code of quotient(x, s) (reciprocal + one residual step) must equal the code of div.rn(x, s) for

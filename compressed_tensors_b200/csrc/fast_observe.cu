@@ -71,35 +71,29 @@ struct ObserveQuantPackOp {
     }
 };
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fused observer kernel for dtype=%d bits=%d asym=%d lanes/group=%d", sig.p_dt, sig.sel, sig.zp, sig.group); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
 template <class P, int BITS, int ASYM>
-static int observe_lpg(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.group) {
-    case 1: return launch_stream<ObserveQuantPackOp<P, BITS, ASYM, 1>>(lp, device, st);
-    case 2: return launch_stream<ObserveQuantPackOp<P, BITS, ASYM, 2>>(lp, device, st);
-    case 4: return launch_stream<ObserveQuantPackOp<P, BITS, ASYM, 4>>(lp, device, st);
-    case 8: return launch_stream<ObserveQuantPackOp<P, BITS, ASYM, 8>>(lp, device, st);
+static StreamKernel observe_lpg(int lanes_per_group) {
+    switch (lanes_per_group) {
+    case 1: return stream_kernel<ObserveQuantPackOp<P, BITS, ASYM, 1>>();
+    case 2: return stream_kernel<ObserveQuantPackOp<P, BITS, ASYM, 2>>();
+    case 4: return stream_kernel<ObserveQuantPackOp<P, BITS, ASYM, 4>>();
+    case 8: return stream_kernel<ObserveQuantPackOp<P, BITS, ASYM, 8>>();
     }
-    SIG_FAIL(s);
+    return {};
 }
 template <class P>
-static int observe_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == 4 && s.zp == 0) return observe_lpg<P, 4, 0>(s, lp, device, st);
-    if (s.sel == 4 && s.zp == 1) return observe_lpg<P, 4, 1>(s, lp, device, st);
-    if (s.sel == 8 && s.zp == 0) return observe_lpg<P, 8, 0>(s, lp, device, st);
-    if (s.sel == 8 && s.zp == 1) return observe_lpg<P, 8, 1>(s, lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel observe_p(int bits, bool asym, int lanes_per_group) {
+    if (bits == 4 && !asym) return observe_lpg<P, 4, 0>(lanes_per_group);
+    if (bits == 4 && asym) return observe_lpg<P, 4, 1>(lanes_per_group);
+    if (bits == 8 && !asym) return observe_lpg<P, 8, 0>(lanes_per_group);
+    if (bits == 8 && asym) return observe_lpg<P, 8, 1>(lanes_per_group);
+    return {};
 }
 
-int launch_fast_observe(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.p_dt == CT_BF16) return observe_p<BF16>(s, lp, device, st);
-    if (s.p_dt == CT_F16) return observe_p<F16>(s, lp, device, st);
-    SIG_FAIL(s);
+StreamKernel observe_kernel(int p_dt, int bits, bool asym, int lanes_per_group) {
+    if (p_dt == CT_BF16) return observe_p<BF16>(bits, asym, lanes_per_group);
+    if (p_dt == CT_F16) return observe_p<F16>(bits, asym, lanes_per_group);
+    return {};
 }
 
 }  // namespace ctb

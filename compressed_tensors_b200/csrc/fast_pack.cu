@@ -5,64 +5,55 @@
 
 namespace ctb {
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fast kernel for op=%d dtype=%d sel=%d zp=%d group=%d", sig.op, sig.p_dt, sig.sel, sig.zp, sig.group); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
-// unit sizes: 4-bit codes -> 4 chunks (32 elements -> 16 B out); 8-bit codes -> 2 chunks
+// unit sizes: 4-bit codes -> 4 chunks (32 elements -> 16 B out); 8-bit codes -> 2 chunks; fp32 -> 1 chunk
 template <class P, int BITS, int ZP>
-static int quantpack_g(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
+static StreamKernel quantpack_u(int max_unit) {
     constexpr int GMAX = (BITS == 4) ? 4 : 2;
     if constexpr (P::DT != CT_F32) {
-        if (s.group == GMAX) return launch_stream<QuantPackOp<P, BITS, ZP, GMAX>>(lp, device, st);
+        if (max_unit >= GMAX) return stream_kernel<QuantPackOp<P, BITS, ZP, GMAX>>();
     }
-    if (s.group == 1) return launch_stream<QuantPackOp<P, BITS, ZP, 1>>(lp, device, st);
-    SIG_FAIL(s);
+    return stream_kernel<QuantPackOp<P, BITS, ZP, 1>>();
 }
 template <class P>
-static int quantpack_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == 4 && s.zp == 0) return quantpack_g<P, 4, 0>(s, lp, device, st);
-    if (s.sel == 4 && s.zp == 1) return quantpack_g<P, 4, 1>(s, lp, device, st);
-    if (s.sel == 8 && s.zp == 0) return quantpack_g<P, 8, 0>(s, lp, device, st);
-    if (s.sel == 8 && s.zp == 1) return quantpack_g<P, 8, 1>(s, lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel quantpack_p(int bits, int zp_kind, int max_unit) {
+    if (bits == 4 && zp_kind == 0) return quantpack_u<P, 4, 0>(max_unit);
+    if (bits == 4 && zp_kind == 1) return quantpack_u<P, 4, 1>(max_unit);
+    if (bits == 8 && zp_kind == 0) return quantpack_u<P, 8, 0>(max_unit);
+    if (bits == 8 && zp_kind == 1) return quantpack_u<P, 8, 1>(max_unit);
+    return {};
 }
-int fast_group_quantpack(int p_dt, int bits) { return p_dt == CT_F32 ? 1 : (bits == 4 ? 4 : 2); }
-
-int launch_fast_quantpack(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.p_dt) {
-    case CT_BF16: return quantpack_p<BF16>(s, lp, device, st);
-    case CT_F16: return quantpack_p<F16>(s, lp, device, st);
-    case CT_F32: return quantpack_p<F32>(s, lp, device, st);
+StreamKernel quantpack_kernel(int p_dt, int bits, int zp_kind, int max_unit) {
+    switch (p_dt) {
+    case CT_BF16: return quantpack_p<BF16>(bits, zp_kind, max_unit);
+    case CT_F16: return quantpack_p<F16>(bits, zp_kind, max_unit);
+    case CT_F32: return quantpack_p<F32>(bits, zp_kind, max_unit);
     }
-    SIG_FAIL(s);
+    return {};
 }
 
 template <class P>
-static int unpackdeq_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.sel == 4 && s.zp == 0) return launch_stream<UnpackDequantOp<P, 4, 0>>(lp, device, st);
-    if (s.sel == 4 && s.zp == 1) return launch_stream<UnpackDequantOp<P, 4, 1>>(lp, device, st);
-    if (s.sel == 8 && s.zp == 0) return launch_stream<UnpackDequantOp<P, 8, 0>>(lp, device, st);
-    if (s.sel == 8 && s.zp == 1) return launch_stream<UnpackDequantOp<P, 8, 1>>(lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel unpackdeq_p(int bits, int zp_kind) {
+    if (bits == 4 && zp_kind == 0) return stream_kernel<UnpackDequantOp<P, 4, 0>>();
+    if (bits == 4 && zp_kind == 1) return stream_kernel<UnpackDequantOp<P, 4, 1>>();
+    if (bits == 8 && zp_kind == 0) return stream_kernel<UnpackDequantOp<P, 8, 0>>();
+    if (bits == 8 && zp_kind == 1) return stream_kernel<UnpackDequantOp<P, 8, 1>>();
+    return {};
 }
-int launch_fast_unpackdeq(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.p_dt) {
-    case CT_BF16: return unpackdeq_p<BF16>(s, lp, device, st);
-    case CT_F16: return unpackdeq_p<F16>(s, lp, device, st);
-    case CT_F32: return unpackdeq_p<F32>(s, lp, device, st);
+StreamKernel unpackdeq_kernel(int p_dt, int bits, int zp_kind) {
+    switch (p_dt) {
+    case CT_BF16: return unpackdeq_p<BF16>(bits, zp_kind);
+    case CT_F16: return unpackdeq_p<F16>(bits, zp_kind);
+    case CT_F32: return unpackdeq_p<F32>(bits, zp_kind);
     }
-    SIG_FAIL(s);
+    return {};
 }
 
-int launch_fast_bits(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.op == F_PACK && s.sel == 4) return launch_stream<PackOp<4>>(lp, device, st);
-    if (s.op == F_PACK && s.sel == 8) return launch_stream<PackOp<8>>(lp, device, st);
-    if (s.op == F_UNPACK && s.sel == 4) return launch_stream<UnpackOp<4>>(lp, device, st);
-    if (s.op == F_UNPACK && s.sel == 8) return launch_stream<UnpackOp<8>>(lp, device, st);
-    SIG_FAIL(s);
+StreamKernel bits_kernel(bool pack, int bits) {
+    if (pack && bits == 4) return stream_kernel<PackOp<4>>();
+    if (pack && bits == 8) return stream_kernel<PackOp<8>>();
+    if (!pack && bits == 4) return stream_kernel<UnpackOp<4>>();
+    if (!pack && bits == 8) return stream_kernel<UnpackOp<8>>();
+    return {};
 }
 
 }  // namespace ctb

@@ -4,62 +4,54 @@
 
 namespace ctb {
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fast kernel for op=%d dtype=%d sel=%d zp=%d group=%d", sig.op, sig.p_dt, sig.sel, sig.zp, sig.group); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
+// the NARROW / WIDE integer kinds share one kernel here
 template <class P, int KIND, int ZP>
-static int quant_g(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
+static StreamKernel quant_u(int max_unit) {
     if constexpr (P::DT != CT_F32) {
-        if (s.group == 2) return launch_stream<QuantizeOp<P, KIND, ZP, 2>>(lp, device, st);
+        if (max_unit >= 2) return stream_kernel<QuantizeOp<P, KIND, ZP, 2>>();
     }
-    if (s.group == 1) return launch_stream<QuantizeOp<P, KIND, ZP, 1>>(lp, device, st);
-    SIG_FAIL(s);
+    return stream_kernel<QuantizeOp<P, KIND, ZP, 1>>();
 }
 template <class P>
-static int quant_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    // the NARROW / WIDE integer kinds share one kernel here
-    const int kind = (s.sel == QF8) ? QF8 : QI_WIDE;
-    if (kind == QF8 && s.zp == 0) return quant_g<P, QF8, 0>(s, lp, device, st);
-    if (kind == QF8 && s.zp == 1) return quant_g<P, QF8, 1>(s, lp, device, st);
-    if (kind == QF8 && s.zp == 2) return quant_g<P, QF8, 2>(s, lp, device, st);   // float8_e4m3fn zero point (the FP8 presets)
-    if (kind == QI_WIDE && s.zp == 0) return quant_g<P, QI_WIDE, 0>(s, lp, device, st);
-    if (kind == QI_WIDE && s.zp == 1) return quant_g<P, QI_WIDE, 1>(s, lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel quant_p(bool fp8, int zp_kind, int max_unit) {
+    if (fp8 && zp_kind == 0) return quant_u<P, QF8, 0>(max_unit);
+    if (fp8 && zp_kind == 1) return quant_u<P, QF8, 1>(max_unit);
+    if (fp8 && zp_kind == 2) return quant_u<P, QF8, 2>(max_unit);   // float8_e4m3fn zero point (the FP8 presets)
+    if (!fp8 && zp_kind == 0) return quant_u<P, QI_WIDE, 0>(max_unit);
+    if (!fp8 && zp_kind == 1) return quant_u<P, QI_WIDE, 1>(max_unit);
+    return {};
 }
-int fast_group_quant(int p_dt) { return p_dt == CT_F32 ? 1 : 2; }
-
-int launch_fast_quant(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.p_dt) {
-    case CT_BF16: return quant_p<BF16>(s, lp, device, st);
-    case CT_F16: return quant_p<F16>(s, lp, device, st);
-    case CT_F32: return quant_p<F32>(s, lp, device, st);
+StreamKernel quant_kernel(int p_dt, bool fp8, int zp_kind, int max_unit) {
+    switch (p_dt) {
+    case CT_BF16: return quant_p<BF16>(fp8, zp_kind, max_unit);
+    case CT_F16: return quant_p<F16>(fp8, zp_kind, max_unit);
+    case CT_F32: return quant_p<F32>(fp8, zp_kind, max_unit);
     }
-    SIG_FAIL(s);
+    return {};
 }
 
 template <class P>
-static int dequant_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if constexpr (P::DT != CT_F32) {
-        if (s.sel == 3 && s.zp == 0) return launch_stream<DequantF32ScaleOp<P>>(lp, device, st);   // fp8 codes, float32 scale, 16-bit output
+static StreamKernel dequant_p(bool fp8, int zp_kind, bool f32_scale) {
+    if (f32_scale) {
+        if constexpr (P::DT != CT_F32) {
+            if (fp8 && zp_kind == 0) return stream_kernel<DequantF32ScaleOp<P>>();
+        }
+        return {};
     }
-    const int kind = (s.sel == QF8) ? QF8 : QI_WIDE;
-    if (kind == QF8 && s.zp == 0) return launch_stream<DequantizeOp<P, QF8, 0>>(lp, device, st);
-    if (kind == QF8 && s.zp == 1) return launch_stream<DequantizeOp<P, QF8, 1>>(lp, device, st);
-    if (kind == QF8 && s.zp == 2) return launch_stream<DequantizeOp<P, QF8, 2>>(lp, device, st);
-    if (kind == QI_WIDE && s.zp == 0) return launch_stream<DequantizeOp<P, QI_WIDE, 0>>(lp, device, st);
-    if (kind == QI_WIDE && s.zp == 1) return launch_stream<DequantizeOp<P, QI_WIDE, 1>>(lp, device, st);
-    SIG_FAIL(s);
+    if (fp8 && zp_kind == 0) return stream_kernel<DequantizeOp<P, QF8, 0>>();
+    if (fp8 && zp_kind == 1) return stream_kernel<DequantizeOp<P, QF8, 1>>();
+    if (fp8 && zp_kind == 2) return stream_kernel<DequantizeOp<P, QF8, 2>>();
+    if (!fp8 && zp_kind == 0) return stream_kernel<DequantizeOp<P, QI_WIDE, 0>>();
+    if (!fp8 && zp_kind == 1) return stream_kernel<DequantizeOp<P, QI_WIDE, 1>>();
+    return {};
 }
-int launch_fast_dequant(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    switch (s.p_dt) {
-    case CT_BF16: return dequant_p<BF16>(s, lp, device, st);
-    case CT_F16: return dequant_p<F16>(s, lp, device, st);
-    case CT_F32: return dequant_p<F32>(s, lp, device, st);
+StreamKernel dequant_kernel(int p_dt, bool fp8, int zp_kind, bool f32_scale) {
+    switch (p_dt) {
+    case CT_BF16: return dequant_p<BF16>(fp8, zp_kind, f32_scale);
+    case CT_F16: return dequant_p<F16>(fp8, zp_kind, f32_scale);
+    case CT_F32: return dequant_p<F32>(fp8, zp_kind, f32_scale);
     }
-    SIG_FAIL(s);
+    return {};
 }
 
 }  // namespace ctb

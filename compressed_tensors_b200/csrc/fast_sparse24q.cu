@@ -106,25 +106,19 @@ struct Sparse24UnpackDequantOp {
     }
 };
 
-#define SIG_FAIL(sig)                                                                              \
-    do {                                                                                           \
-        set_error("no fused 2:4 + int4 kernel for op=%d dtype=%d zp=%d", sig.op, sig.p_dt, sig.zp); \
-        return CT_E_UNSUPPORTED;                                                                   \
-    } while (0)
-
 template <class P>
-static int s24_p(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.op == F_S24_QUANTPACK && s.zp == 0) return launch_stream<Sparse24QuantPackOp<P, 0>>(lp, device, st);
-    if (s.op == F_S24_QUANTPACK && s.zp == 1) return launch_stream<Sparse24QuantPackOp<P, 1>>(lp, device, st);
-    if (s.op == F_S24_UNPACKDEQ && s.zp == 0) return launch_stream<Sparse24UnpackDequantOp<P, 0>>(lp, device, st);
-    if (s.op == F_S24_UNPACKDEQ && s.zp == 1) return launch_stream<Sparse24UnpackDequantOp<P, 1>>(lp, device, st);
-    SIG_FAIL(s);
+static StreamKernel s24_p(bool compress, int zp_kind) {
+    if (compress && zp_kind == 0) return stream_kernel<Sparse24QuantPackOp<P, 0>>();
+    if (compress && zp_kind == 1) return stream_kernel<Sparse24QuantPackOp<P, 1>>();
+    if (!compress && zp_kind == 0) return stream_kernel<Sparse24UnpackDequantOp<P, 0>>();
+    if (!compress && zp_kind == 1) return stream_kernel<Sparse24UnpackDequantOp<P, 1>>();
+    return {};
 }
 
-int launch_fast_sparse24q(const FastSig& s, const LaunchPlan& lp, int device, cudaStream_t st) {
-    if (s.p_dt == CT_BF16) return s24_p<BF16>(s, lp, device, st);
-    if (s.p_dt == CT_F16) return s24_p<F16>(s, lp, device, st);
-    SIG_FAIL(s);
+StreamKernel sparse24q_kernel(bool compress, int p_dt, int zp_kind) {
+    if (p_dt == CT_BF16) return s24_p<BF16>(compress, zp_kind);
+    if (p_dt == CT_F16) return s24_p<F16>(compress, zp_kind);
+    return {};
 }
 
 }  // namespace ctb

@@ -195,12 +195,7 @@ __global__ void __launch_bounds__(BM_THREADS) observe_quantize_mx_kernel(const B
 // ------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------
-// while a stream is being captured the job table travels as kernel parameters (a pageable copy cannot be captured)
-constexpr int UPLOAD_JOBS = 24;
-struct BmJobBlock { BmJob j[UPLOAD_JOBS]; };
-static __global__ void upload_bm_jobs_kernel(BmJob* dst, const __grid_constant__ BmJobBlock blk, int n) {
-    if ((int)threadIdx.x < n) dst[threadIdx.x] = blk.j[threadIdx.x];
-}
+constexpr int UPLOAD_JOBS = 24;   // jobs per kernel-parameter block of a captured table upload (upload_jobs, common.cuh)
 
 static bool is_inf_div(int64_t v) { return v == CT_DIV_INF; }
 
@@ -284,19 +279,8 @@ int run_observe_block_mx(int op, int n, const ct_quant_desc* descs, const void* 
     if (jobs.size() > 1) {
         rc = scratch_alloc(reinterpret_cast<void**>(&table), jobs.size() * sizeof(BmJob), device, st);
         if (rc) return rc;
-        cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
-        cudaStreamIsCapturing(st, &capturing);
-        if (capturing == cudaStreamCaptureStatusActive) {
-            for (size_t o = 0; o < jobs.size(); o += UPLOAD_JOBS) {
-                BmJobBlock blk;
-                const int cnt = (int)(jobs.size() - o < (size_t)UPLOAD_JOBS ? jobs.size() - o : UPLOAD_JOBS);
-                memcpy(blk.j, jobs.data() + o, (size_t)cnt * sizeof(BmJob));
-                upload_bm_jobs_kernel<<<1, 32, 0, st>>>(table + o, blk, cnt);
-            }
-            count_launch((int)((jobs.size() + UPLOAD_JOBS - 1) / UPLOAD_JOBS));
-        } else {
-            CT_CUDA_TRY(cudaMemcpyAsync(table, jobs.data(), jobs.size() * sizeof(BmJob), cudaMemcpyHostToDevice, st));
-        }
+        rc = upload_jobs<BmJob, UPLOAD_JOBS>(reinterpret_cast<uint8_t*>(table), 0, jobs.data(), jobs.size(), st);
+        if (rc) return rc;
     }
     if (block) observe_quantize_block_kernel<<<(unsigned)ctas, BM_THREADS, 0, st>>>(table, (int)jobs.size(), jobs[0]);
     else observe_quantize_mx_kernel<<<(unsigned)ctas, BM_THREADS, 0, st>>>(table, (int)jobs.size(), jobs[0]);

@@ -17,6 +17,12 @@ struct F32 {
 };
 
 enum QKind { QI_NARROW = 0, QI_WIDE = 1, QF8 = 2 };
+// rounding kind of fake_quantize on compute dtype p_dt: the packed magic-number rounding in T (QI_NARROW) covers codes of up to 7 bits
+// in bf16 and 8 in fp16; wider codes and fp32 round through rintf (QI_WIDE)
+inline int fake_kind(int p_dt, int qtype, int bits) {
+    if (qtype == CT_Q_FLOAT) return QF8;
+    return (p_dt == CT_F32 || bits > (p_dt == CT_BF16 ? 7 : 8)) ? QI_WIDE : QI_NARROW;
+}
 
 template <class P> struct ElemBytes { static constexpr int v = 2; };
 template <> struct ElemBytes<F32> { static constexpr int v = 4; };
@@ -120,7 +126,7 @@ __device__ __forceinline__ void store_words(uint8_t* p, const uint32_t (&o)[N]) 
 template <class P, int BITS, int ZP, int G>
 struct QuantPackOp {
     static_assert(BITS == 4 || BITS == 8, "fast path packs 4- and 8-bit codes");
-    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
+    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
     static constexpr bool INPUT_EVICT_FIRST = false;   // reads 2-8x what it writes: see InputEvictFirst
@@ -185,7 +191,7 @@ struct QuantPackOp {
 // ------------------------------------------------------------------------------------
 template <class P, int KIND, int ZP, int G>
 struct QuantizeOp {
-    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
+    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
     static constexpr int IN_BYTES = 8 * ElemBytes<P>::v;
@@ -276,7 +282,7 @@ __device__ __forceinline__ void store_out8(uint8_t* out, uint32_t gc, const uint
 // ------------------------------------------------------------------------------------
 template <class P, int KIND /* QI_* = int8 codes, QF8 = e4m3 codes */, int ZP>
 struct DequantizeOp {
-    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
+    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
     static constexpr int IN_BYTES = 8;
@@ -324,7 +330,7 @@ struct DequantizeOp {
 // ------------------------------------------------------------------------------------
 template <class P>
 struct DequantF32ScaleOp {
-    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
+    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
     static constexpr int IN_BYTES = 8;
@@ -354,7 +360,7 @@ struct DequantF32ScaleOp {
 template <class P, int BITS, int ZP>
 struct UnpackDequantOp {
     static_assert(BITS == 4 || BITS == 8, "fast path unpacks 4- and 8-bit codes");
-    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;   // engine.h: sig_tile_chunks
+    static constexpr int TILE = (P::DT == CT_F32) ? TILE_CHUNKS : BIG_TILE_CHUNKS;
     static constexpr int PREF_STAGES = (P::DT == CT_F32) ? 4 : 3;
     static constexpr int PREF_CTAS = (P::DT == CT_F32) ? 3 : 2;
     static constexpr int IN_BYTES = BITS;

@@ -25,8 +25,7 @@ namespace ctb {
 
 constexpr int TILE_CHUNKS = 1024;   // default tile: 1024 chunks = 8192 elements (16 KB of bf16)
 // An op may ask for another tile size (`static constexpr int TILE`).  The four headline 16-bit ops run on 2048-chunk tiles with a
-// 3-stage x 2-CTA ring: half the per-tile bookkeeping of the consumer warps for the same bytes in flight.  The host side must
-// count tiles with the same number: sig_tile_chunks() in engine.h, checked at every launch.
+// 3-stage x 2-CTA ring: half the per-tile bookkeeping of the consumer warps for the same bytes in flight.
 constexpr int BIG_TILE_CHUNKS = 2048;
 constexpr int CHUNK_ELEMS = 8;
 constexpr int NCW = 8;              // consumer warps
@@ -324,7 +323,6 @@ struct LaunchPlan {
     JobTable tbl;
     Common cm;
     uint32_t total_tiles;
-    int tile_chunks = TILE_CHUNKS;   // the tile size the host counted tiles with; must equal TileOf<Op>::value of the kernel launched
     uint32_t* sched = nullptr;   // zeroed device counter for the dynamic tile schedule (nullptr = static deal); owned by dispatch.cu
 };
 
@@ -351,10 +349,6 @@ constexpr RingShape ring_shape() {
 template <class Op>
 int launch_stream(const LaunchPlan& lp, int device, cudaStream_t stream) {
     if (lp.total_tiles == 0) return CT_OK;
-    if (lp.tile_chunks != TileOf<Op>::value) {
-        set_error("internal: tiles counted with %d chunks, the kernel uses %d", lp.tile_chunks, TileOf<Op>::value);
-        return CT_E_ARG;
-    }
     constexpr size_t TILE_BYTES = (size_t)TileOf<Op>::value * Op::IN_BYTES;
     constexpr RingShape ring = ring_shape<Op>();
     static_assert(ring_fits(ring, TILE_BYTES), "the op's tile does not fit a ring in 200 KB of shared memory");
@@ -368,5 +362,14 @@ int launch_stream(const LaunchPlan& lp, int device, cudaStream_t stream) {
     CT_CUDA_TRY(cudaGetLastError());
     return CT_OK;
 }
+
+// A streaming kernel as the host plans it: its launcher and the tile size the host counts the launch's tiles in.
+// A null `launch` means there is no instantiation for what was asked.
+struct StreamKernel {
+    int (*launch)(const LaunchPlan&, int device, cudaStream_t);
+    int tile_chunks;
+};
+template <class Op>
+constexpr StreamKernel stream_kernel() { return {&launch_stream<Op>, TileOf<Op>::value}; }
 
 }  // namespace ctb

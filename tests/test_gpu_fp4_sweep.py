@@ -7,7 +7,7 @@ scale) are undefined in the reference and not compared; fake-quantized and dequa
 Each encode and decode sweep runs three ways, so that both kernels are checked and the test knows which one ran:
   fast     a layout the streaming planner takes (cols % 32 == 0, 16-byte aligned);
   generic  the same data as a view 2 bytes past an aligned allocation, which the planner must send to the generic kernel;
-  batched  one ops.batched call holding one entry of each, which must make exactly 2 launches (one per signature, one per generic
+  batched  one ops.batched call holding one entry of each, which must make exactly 2 launches (one per streaming kernel, one per generic
            tensor), proving the aligned entry took the streaming kernel and the offset one did not.
 
 Kernel branches and the tests that reach them:

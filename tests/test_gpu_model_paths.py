@@ -1,16 +1,16 @@
 """
 The paths a whole model takes, element by element against the CPU oracle:
 
-  A. mixed multi-tensor job tables (ct_batched through ops.batched / ops.BatchedPlan): several kernel signatures, flat and 2-D
+  A. mixed multi-tensor job tables (ct_batched through ops.batched / ops.BatchedPlan): several streaming kernels, flat and 2-D
      scale addressing, partial and single-chunk tiles, unit-size fallbacks, misaligned views and empty tensors in ONE call;
   B. what those tables cover of the ring shapes and tile schedules the library launches with, and a CUDA-graph replay;
   C. the host-resident pipeline ct_host_run_many: one large CPU tensor through the per-tensor ops (chunked), a CPU-resident model
      through ops.host_batched (chunks of many tensors sharing staging slots, an error part-way) and ModelCompressor on a
      CPU-resident model.
 
-Every table entry names the kernel it is meant to take (a signature label, "generic" or "empty").  The number of launches a
+Every table entry names the kernel it is meant to take (a kernel label, "generic" or "empty").  The number of launches a
 call makes is written next to each table, derived by hand from the planner's rules in csrc/dispatch.cu (plan_one / plan_fp4 /
-plan_s24): one launch per distinct signature, one per generic tensor, none for an empty tensor.  The count is what shows that
+plan_s24): one launch per distinct kernel, one per generic tensor, none for an empty tensor.  The count is what shows that
 the table really took the paths it is meant to cover.
 """
 import math
@@ -181,23 +181,23 @@ def _check(outs, wants, specs, what):
 
 # --------------------------------------------------------------------------------------------
 # A. the mixed tables of ops 0-4.  Tile: 2048 chunks (16384 elements) for 16-bit quantize+pack, unpack+dequantize, quantize and
-# dequantize, 1024 chunks (8192 elements) otherwise (engine.h: sig_tile_chunks).  A "unit" is sig.group chunks of 8 elements.
+# dequantize, 1024 chunks (8192 elements) otherwise (the functors' TILE in csrc/ops.cuh).  A "unit" is one thread's 1, 2 or 4 chunks of 8 elements.
 # --------------------------------------------------------------------------------------------
 def _many(label, dt, bits=4, **kw):
-    """34 more jobs of one signature: together with the table's own entries more than 32 jobs in that group (two table blocks)"""
+    """34 more jobs of one kernel: together with the table's own entries more than 32 jobs in that group (two table blocks)"""
     return [S(label, (8 * k, 256 + 128 * (k % 3)), dt, "group", 128, bits=bits, **kw) for k in range(1, 35)]
 
 
-# op 0, quantize + pack.  Signature (x dtype, bits, zero point, unit): A1 = bf16/4/-/1, A4 = bf16/4/-/4, A4z = bf16/4/int8/4,
-# B2z = fp16/8/int8/2, C1 = fp32/4/-/1, C8 = fp32/8/-/1.  6 signatures + 5 generic tensors = 11 launches.
+# op 0, quantize + pack.  Kernel (x dtype, bits, zero point, unit): A1 = bf16/4/-/1, A4 = bf16/4/-/4, A4z = bf16/4/int8/4,
+# B2z = fp16/8/int8/2, C1 = fp32/4/-/1, C8 = fp32/8/-/1.  6 kernels + 5 generic tensors = 11 launches.
 T_QPACK = [
     S("A1", (1, 8), BF, "tensor"),                                   # 8 elements: one chunk, unit falls back to 1 chunk
     S("A4", (16, 1024), BF, "group", 128),                           # exactly one tile
     S("A4", (19, 864), BF, "channel"),                               # one tile + one unit (2052 chunks)
     S("A4", (73, 224), BF, "group1", 32),                            # one tile - one unit (2044 chunks), one row of group scales (2-D)
-    S("A1", (32, 64), BF, "group", 8),                               # group of one chunk: sig.group = 1
+    S("A1", (32, 64), BF, "group", 8),                               # group of one chunk: unit = 1 chunk
     S("A4z", (128, 256), BF, "block", (64, 64), zp=torch.int8),      # blocks that divide the tensor
-    S("A1", (100, 200), BF, "block", (64, 64)),                      # blocks that do not: 25 chunks a row, sig.group = 1
+    S("A1", (100, 200), BF, "block", (64, 64)),                      # blocks that do not: 25 chunks a row, unit = 1 chunk
     S("B2z", (64, 512), FP16, "channel", bits=8, zp=torch.int8),
     S("C1", (48, 256), FP32, "group", 128),
     S("C1", (896, 8192), FP32, "group", 128),                        # 896 tiles: wraps the 2-stage ring, static deal (section B)
@@ -216,7 +216,7 @@ L_QPACK = 11
 L_QPACK_CAPTURED = L_QPACK + 4
 
 # op 1, unpack + dequantize (no unit grouping; the 4-bit input of a job must be a multiple of 16 bytes for the bulk copy).
-# U4 = bf16/4/-, U4z = bf16/4/int8, V8z = fp16/8/int8, W4 = fp32/4/-.  4 signatures + 7 generic = 11 launches.
+# U4 = bf16/4/-, U4z = bf16/4/int8, V8z = fp16/8/int8, W4 = fp32/4/-.  4 kernels + 7 generic = 11 launches.
 T_UNPACK = [
     S("generic", (1, 8), BF, "tensor"),                              # one chunk = 4 bytes of packed input: generic
     S("U4", (1, 32), BF, "tensor"),                                  # 4 chunks = 16 bytes: the smallest streamed job
@@ -242,13 +242,13 @@ L_UNPACK = 11
 
 # op 2, quantize (unit 2 chunks for 16-bit x).  Signature (x dtype, kind, zero point, unit, bits):
 # Q1 = bf16/int/-/1/8, Q2 = bf16/int/-/2/8, Q2b4 = bits 4, Q2b3 = bits 3, Q2z / Q1z = int8 zero point, F2z8 = bf16/fp8/fp8 zp/2,
-# G2 = fp16/fp8/-/2, R1 = fp32/int/-/1/8.  9 signatures + 4 generic = 13 launches.
+# G2 = fp16/fp8/-/2, R1 = fp32/int/-/1/8.  9 kernels + 4 generic = 13 launches.
 T_QUANT = [
     S("Q1", (1, 8), BF, "tensor", bits=8),
     S("Q2", (16, 1024), BF, "group", 128, bits=8),
     S("Q2", (25, 656), BF, "channel", bits=8),                       # one tile + one unit (2050 chunks)
     S("Q2", (31, 528), BF, "group1", 16, bits=8),                    # one tile - one unit (2046 chunks)
-    S("Q1", (32, 64), BF, "group", 8, bits=8),                       # sig.group = 1
+    S("Q1", (32, 64), BF, "group", 8, bits=8),                       # unit = 1 chunk
     S("Q2b4", (32, 128), BF, "tensor", bits=4),
     S("Q2b3", (8, 96), BF, "tensor", bits=3),                        # any width streams here: only the clamp bounds change
     S("F2z8", (64, 256), BF, "tensor", bits=8, qtype="float", zp=F8),
@@ -267,7 +267,7 @@ L_QUANT = 13
 
 # op 3, dequantize (one-byte codes: a job must be an even number of chunks, 16 bytes, for the bulk copy).  D = bf16/int8 codes/-,
 # Dz = int8 zero point, E8z = bf16/fp8 codes/fp8 zp, S3 = fp8 codes, float32 scale, bf16 output, H = fp16/int8, J = fp32/int8.
-# 6 signatures + 7 generic = 13 launches.
+# 6 kernels + 7 generic = 13 launches.
 T_DEQUANT = [
     S("generic", (1, 8), BF, "tensor"),                              # one chunk = 8 bytes of codes
     S("D", (1, 16), BF, "tensor"),                                   # two chunks: the smallest streamed job
@@ -292,7 +292,7 @@ T_DEQUANT = [
 L_DEQUANT = 13
 
 # op 4, fake_quantize (1024-chunk tiles).  K4 = bf16/narrow int/-/4 bits, K4z = int8 zp, K3 = 3 bits, K8 = bf16/wide int/-/8,
-# L8z = fp16/int8 zp/8 bits, M = bf16/fp8/fp8 zp, P4 = fp32/4 bits.  7 signatures + 4 generic = 11 launches.
+# L8z = fp16/int8 zp/8 bits, M = bf16/fp8/fp8 zp, P4 = fp32/4 bits.  7 kernels + 4 generic = 11 launches.
 T_FAKE = [
     S("K4", (1, 8), BF, "tensor"),
     S("K4", (8, 1024), BF, "group", 128),                            # exactly one tile
@@ -359,13 +359,13 @@ def _run_table(t, what):
 
 
 def test_tables_name_the_paths_they_count():
-    """the launch counts written next to the tables agree with their labels (one per signature, one per generic tensor)"""
+    """the launch counts written next to the tables agree with their labels (one per kernel, one per generic tensor)"""
     for name, (_, table, n) in TABLES.items():
         labels = [s.label for s in table]
         assert len(table) >= 40, name
         fast = {l for l in labels if l not in ("generic", "empty")}
         assert n == len(fast) + labels.count("generic"), name
-        assert max(labels.count(l) for l in fast) > 32, f"{name}: no signature group with more than 32 jobs"
+        assert max(labels.count(l) for l in fast) > 32, f"{name}: no kernel group with more than 32 jobs"
     for labels, n in (([e[1] for e in T_FP4], L_FP4), ([e[0] for e in T_FP4D], L_FP4D)):
         assert n == len(set(labels) - {"generic", "empty"}) + labels.count("generic")
 
@@ -386,9 +386,9 @@ def _mx_scale(x, group):
     return torch.exp2(e).to(x.dtype)
 
 
-# op 8, quantize + pack to FP4.  NV signatures (x dtype, scale kind, zero point): N1 = bf16/bf16 scale/-, N2 = bf16/float32 scale/-,
+# op 8, quantize + pack to FP4.  NV kernels (x dtype, scale kind, zero point): N1 = bf16/bf16 scale/-, N2 = bf16/float32 scale/-,
 # N2z = bf16/float32 scale/fp8 zp, O1 = fp16/fp16 scale/-.  MX (group 32 / 64, arithmetic in x's dtype): X0 = bf16/-, X2 = bf16/uint8 zp,
-# Y3 = fp16/int8 zp.  Every NV tensor has its own global scale (Job.aux).  7 signatures + 3 generic = 10 launches.
+# Y3 = fp16/int8 zp.  Every NV tensor has its own global scale (Job.aux).  7 kernels + 3 generic = 10 launches.
 # (kind, label, shape, x dtype, scale dtype, group, zero point dtype, magnitude of x)
 T_FP4 = [
     ("nv", "N1", (8, 1024), BF, BF, 16, None, 1.0),                  # exactly one tile (1024 chunks)
@@ -445,9 +445,9 @@ def _fp4_problem(entry, g, device=DEV):
 
 
 # op 9, unpack + dequantize FP4 (bulk copies need n % 32 == 0).  Signatures (output dtype, scale kind): Sb = bf16/bf16 scale,
-# F8b = bf16/stored fp8, E8b = bf16/stored E8M0, Sh = fp16/fp16 scale.  The kernel of a signature does not know whether a job has a
+# F8b = bf16/stored fp8, E8b = bf16/stored E8M0, Sh = fp16/fp16 scale.  The kernel does not know whether a job has a
 # global scale: Sb jobs of 128 tiles with and without one alternate, and the static deal hands each CTA tiles of different jobs
-# (section B).  4 signatures + 1 generic = 5 launches.
+# (section B).  4 kernels + 1 generic = 5 launches.
 # (label, shape, scale kind, output dtype, group, global scale)
 T_FP4D = [("Sb", (512, 2048), "same", BF, 16, (i % 2 == 0)) for i in range(8)] + [
     ("F8b", (64, 256), "fp8", BF, 16, True),
@@ -515,7 +515,7 @@ def test_mixed_fp4_unpack_dequantize_table_vs_oracle():
 
 
 def test_fused_nvfp4_observer_table_vs_oracle():
-    """op 10 over several tensors of very different maxima, bf16 and fp16 (one signature each = 2 launches; the empty one none)"""
+    """op 10 over several tensors of very different maxima, bf16 and fp16 (one kernel each = 2 launches; the empty one none)"""
     from compressed_tensors_b200.quantization import QuantizationArgs
     from compressed_tensors_b200.quantization.utils import calculate_qparams
 
@@ -654,7 +654,7 @@ def test_tables_wrap_every_ring():
             dts.setdefault(s.label, set()).add(s.dt)
         wrapped, static = set(), False
         for label, n in tiles.items():
-            assert len(dts[label]) == 1, f"{name}: signature {label} mixes element types"
+            assert len(dts[label]) == 1, f"{name}: kernel {label} mixes element types"
             tile, stages, ctas = RINGS[(op, dts[label].pop())]
             grid = min(sms * ctas, n)
             if n > grid * stages:
