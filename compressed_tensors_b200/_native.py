@@ -45,6 +45,8 @@ DT = {
 Q_INT, Q_FLOAT, Q_FP4 = 0, 1, 2
 DT_E8M0 = 8  # uint8 MX scale exponent as stored (CT_E8M0)
 DT_F64 = 9   # compute precision of ct_hadamard_transform (CT_F64)
+# bytes per element of each ct_dtype_t a tensor can hold
+DT_SIZE = {code: torch.empty((), dtype=dt).element_size() for dt, code in DT.items()} | {DT_E8M0: 1}
 
 
 class QuantDesc(ctypes.Structure):

@@ -58,36 +58,32 @@ def _fp4_ok(sd, fmt, place, key: str) -> bool:
     return True
 
 
+def _problem(c: "ops._Call", keep: list):
+    """(desc, in, scale, zp, out) of one module's call, its output allocated where its input lives; `keep` holds the call (and the
+    global scale its descriptor points at) until the launch"""
+    out = _empty(c.out_shape, c.out_dtype, c.src)
+    if c.p.gs is not None:
+        c.desc.global_scale = c.p.gs.data_ptr()
+    keep.append(c)
+    return (c.desc, c.src.contiguous(), c.p.scale.contiguous(), c.p.zp.contiguous() if c.p.zp is not None else None, out)
+
+
 def _compress_fp4_group(mods, fmt, place, force_format, host) -> None:
     comp = BaseCompressor.get_value_from_registry(fmt.value)
     probs, staged, keep = [], [], []
     for m in mods:
         scheme = m.quantization_scheme
         scheme.format = fmt
-        args = scheme.weights
         sd = host.get(m) or get_direct_state_dict(m)
-        w, sc = sd["weight"], sd["weight_scale"]
         gs = sd.get("weight_global_scale", None) if fmt == CompressionFormat.nvfp4_pack_quantized else None
         try:
-            if w.shape[1] % 2 != 0:
-                raise ValueError("odd columns")
-            scale, gsv, se = ops._global_scale(sc, gs)
-            qtype, bits = ops._qparams(args)
-            if qtype != N.Q_FP4 or (gs is not None and gsv is None):
-                raise NotImplementedError
-            cd = torch.result_type(w, scale if gsv is None else ops._like(scale, se))
-            zp = sd.get("weight_zero_point", None)
-            p = ops._resolve(w, scale, zp, args, None)
-            d = ops._desc(p, w.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, w.dtype, None, qtype, bits, se)
-            if gsv is not None:
-                d.global_scale = gsv.data_ptr()
-                keep.append(gsv)
-            out = _empty((p.rows, p.cols // 2), torch.uint8, w)
+            c = ops._quantize_pack_fp4_call(sd["weight"], sd["weight_scale"], sd.get("weight_zero_point", None), scheme.weights,
+                                            global_scale=gs)
         except (ValueError, NotImplementedError):
             compress_module(m, force_format)
             continue
-        probs.append((d, w.contiguous(), p.scale.contiguous(), p.zp.contiguous() if p.zp is not None else None, out))
-        staged.append((m, sd, out))
+        probs.append(_problem(c, keep))
+        staged.append((m, sd, probs[-1][4]))
     _run(N.OP_QUANTIZE_PACK_FP4, probs, place)
     for m, sd, out in staged:
         scheme = m.quantization_scheme
@@ -108,31 +104,17 @@ def _decompress_fp4_group(mods, fmt, place, force_format, host) -> None:
         scheme.format = fmt
         sd = host.get(m) or get_direct_state_dict(m)
         packed, sc = sd["weight_packed"], sd["weight_scale"]
-        gs = sd.get("weight_global_scale", None)
         try:
-            if packed.dtype != torch.uint8 or packed.ndim != 2:
-                raise ValueError
-            stored = {torch.float8_e4m3fn: N.DT[torch.float8_e4m3fn], torch.uint8: N.DT_E8M0}.get(sc.dtype)
-            if stored is None or (gs is not None and not (gs.dtype == torch.float32 and gs.numel() == 1 and gs.ndim >= 1)):
-                raise NotImplementedError
-            rows, cols = packed.shape[0], packed.shape[1] * 2
-            like = torch.empty((rows, cols), dtype=torch.int8, device="meta")
-            p = ops._resolve(like, sc, None, ops._infer_dequant_args(like, sc), None)
-            se = torch.float32 if gs is not None else dense
-            d = ops._desc(p, None, torch.float32, None, None, None, dense, N.Q_FP4, 4, se)
-            d.scale_dtype = stored
-            if gs is not None:
-                gsv = gs.reshape(1).contiguous()
-                d.global_scale = gsv.data_ptr()
-                keep.append(gsv)
-            out = _empty((rows, cols), dense, packed)
+            if sc.dtype not in (torch.float8_e4m3fn, torch.uint8):
+                raise NotImplementedError   # only scales stored as the compressor writes them are batched
+            c = ops._unpack_dequantize_fp4_call(packed, sc, sd.get("weight_global_scale", None), dense, comp._stored_scale)
         except (ValueError, NotImplementedError):
             decompress_module(m, force_format)
             continue
-        probs.append((d, packed.contiguous(), p.scale.contiguous(), None, out))
+        probs.append(_problem(c, keep))
         new = sd.copy()
         new.pop("weight_packed")
-        new["weight"] = out
+        new["weight"] = probs[-1][4]
         new["weight_scale"] = comp._decompress_scale(sc, dense)
         staged.append((m, new))
     _run(N.OP_UNPACK_DEQUANTIZE_FP4, probs, place)
@@ -291,7 +273,7 @@ def compress_modules_batched(modules, force_format: Optional[CompressionFormat] 
             continue
         comp = BaseCompressor.get_value_from_registry(fmt.value)
         pack = fmt == CompressionFormat.pack_quantized
-        probs, staged = [], []
+        probs, staged, keep = [], [], []
         for m in mods:
             scheme = m.quantization_scheme
             scheme.format = fmt
@@ -303,21 +285,12 @@ def compress_modules_batched(modules, force_format: Optional[CompressionFormat] 
             # integer), so it is skipped; for fp8 codes -0.0 and +0.0 are different bytes (0x80 / 0x00), so it is added
             zp = sd.get("weight_zero_point", None) if (not args.symmetric or args.type == "float") else None
             try:
-                p = ops._resolve(w, sc, zp, args, None)
-                qtype, bits = ops._qparams(args)
-                cd = torch.result_type(w, sc)
-                if pack:
-                    out = _empty((p.rows, -(-p.cols * bits // 32)), torch.int32, w)
-                    d = ops._desc(p, w.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, torch.int8, None, qtype, bits)
-                else:
-                    qd = args.pytorch_dtype()
-                    out = _empty(w.shape, qd, w)
-                    d = ops._desc(p, w.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, qd, qd, qtype, bits)
+                c = ops._quantize_pack_call(w, sc, zp, args) if pack else ops._quantize_call(w, sc, zp, args, dtype=args.pytorch_dtype())
             except (ValueError, NotImplementedError):
                 compress_module(m, force_format)
                 continue
-            probs.append((d, w.contiguous(), p.scale.contiguous(), p.zp.contiguous() if p.zp is not None else None, out))
-            staged.append((m, sd, out))
+            probs.append(_problem(c, keep))
+            staged.append((m, sd, probs[-1][4]))
         _run(N.OP_QUANTIZE_PACK if pack else N.OP_QUANTIZE, probs, place)
         for m, sd, out in staged:
             scheme = m.quantization_scheme
@@ -344,7 +317,7 @@ def decompress_modules_batched(modules, force_format: Optional[CompressionFormat
             _decompress_fp4_group(mods, fmt, place, force_format, host)
             continue
         pack = fmt == CompressionFormat.pack_quantized
-        probs, staged = [], []
+        probs, staged, keep = [], [], []
         for m in mods:
             scheme = m.quantization_scheme
             scheme.format = fmt
@@ -355,30 +328,19 @@ def decompress_modules_batched(modules, force_format: Optional[CompressionFormat
             new = sd.copy()
             try:
                 if pack:
-                    packed = sd["weight_packed"]
                     shape = tuple(int(v) for v in sd["weight_shape"].tolist())
                     if zp is not None and not args.symmetric and args.strategy in ("group", "channel"):
                         zp = ops.unpack_from_int32(zp, args.num_bits, (*shape[:-1], sc.shape[-1]), packed_dim=0)
                         new["weight_zero_point"] = zp
-                    like = torch.empty(shape, dtype=torch.int8, device="meta")
-                    iargs = ops._infer_dequant_args(like, sc)
-                    p = ops._resolve(like, sc, zp, iargs, None)
-                    out = _empty(shape, sc.dtype, packed)
-                    d = ops._desc(p, None, p.scale.dtype, p.zp.dtype if p.zp is not None else None, None, torch.int8, sc.dtype, N.Q_INT, args.num_bits)
-                    src = packed.contiguous()
+                    c = ops._unpack_dequantize_call(sd["weight_packed"], sc, zp, args.num_bits, shape)
                     new.pop("weight_packed")
                 else:
-                    q = sd["weight"]
-                    iargs = ops._infer_dequant_args(q, sc)
-                    p = ops._resolve(q, sc, zp, iargs, None)
-                    out = _empty(q.shape, sc.dtype, q)
-                    d = ops._desc(p, None, p.scale.dtype, p.zp.dtype if p.zp is not None else None, None, q.dtype, sc.dtype, N.Q_INT, 8)
-                    src = q.contiguous()
+                    c = ops._dequantize_call(sd["weight"], sc, zp)
             except (ValueError, NotImplementedError):
                 decompress_module(m, force_format)
                 continue
-            probs.append((d, src, p.scale.contiguous(), p.zp.contiguous() if p.zp is not None else None, out))
-            new["weight"] = out
+            probs.append(_problem(c, keep))
+            new["weight"] = probs[-1][4]
             staged.append((m, new))
         _run(N.OP_UNPACK_DEQUANTIZE if pack else N.OP_DEQUANTIZE, probs, place)
         for m, new in staged:

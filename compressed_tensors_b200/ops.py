@@ -21,7 +21,7 @@ import ctypes
 import functools
 import math
 import threading
-from typing import Optional, Sequence, Tuple
+from typing import NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -289,53 +289,80 @@ def _check_float(t: torch.Tensor, what: str):
         raise NotImplementedError(f"{what} dtype {t.dtype} is not supported by compressed_tensors_b200 (fp32/fp16/bf16 only)")
 
 
-def _desc(p: _Problem, x_dt, s_dt, zp_dt, cd, q_dt, out_dt, qtype, bits, se_dt=None) -> N.QuantDesc:
-    """se_dt: dtype of scale / global_scale (or, for stored fp8 / E8M0 scales, the float dtype they decode to)"""
-    d = N.QuantDesc()
-    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = p.rows, p.cols, p.rdiv, p.cdiv, p.srs
-    d.x_dtype = N.DT.get(x_dt, N.DT_NONE)
-    d.scale_dtype = N.DT[s_dt]
-    d.zp_dtype = N.DT[zp_dt] if zp_dt is not None else N.DT_NONE
-    d.compute_dtype = N.DT.get(cd, N.DT_NONE)
-    d.q_dtype = N.DT.get(q_dt, N.DT_NONE)
-    d.out_dtype = N.DT.get(out_dt, N.DT_NONE)
-    d.qtype, d.num_bits = qtype, bits
-    d.global_scale = None
-    d.seff_dtype = N.DT.get(se_dt, N.DT_NONE)
-    d.aux = None
+_DT_FIELDS = ("x_dtype", "scale_dtype", "zp_dtype", "compute_dtype", "q_dtype", "out_dtype", "seff_dtype")
+
+
+def _qdesc(rows: int, cols: int, rdiv: int, cdiv: int, srs: int, qtype: int = N.Q_INT, num_bits: int = 0, global_scale=None,
+           **dtypes) -> N.QuantDesc:
+    """a descriptor in which every field the caller does not name is absent: CT_NONE dtypes, no global scale, no aux.
+    dtypes: the `*_dtype` fields, each a torch dtype or a ct_dtype_t code"""
+    d = N.QuantDesc(rows=rows, cols=cols, rdiv=rdiv, cdiv=cdiv, s_row_stride=srs, qtype=qtype, num_bits=num_bits,
+                    global_scale=global_scale)
+    for f in _DT_FIELDS:
+        v = dtypes.pop(f, None)
+        setattr(d, f, N.DT_NONE if v is None else v if isinstance(v, int) else N.DT[v])
+    if dtypes:
+        raise TypeError(f"unknown descriptor fields {sorted(dtypes)}")
     return d
 
 
-def _run(fn_name: str, op: int, d: N.QuantDesc, p: _Problem, src: torch.Tensor, out_shape, out_dtype) -> torch.Tensor:
-    """src: the streamed input tensor (x, q or packed words), already 2-D"""
+def _desc(p: _Problem, x_dt, s_dt, zp_dt, cd, q_dt, out_dt, qtype, bits, se_dt=None) -> N.QuantDesc:
+    """se_dt: dtype of scale / global_scale (or, for stored fp8 / E8M0 scales, the float dtype they decode to)"""
+    def code(t):
+        return N.DT.get(t, N.DT_NONE)
+
+    return _qdesc(p.rows, p.cols, p.rdiv, p.cdiv, p.srs, qtype, bits, x_dtype=code(x_dt), scale_dtype=N.DT[s_dt], zp_dtype=zp_dt,
+                  compute_dtype=code(cd), q_dtype=code(q_dt), out_dtype=code(out_dt), seff_dtype=code(se_dt))
+
+
+class _Call(NamedTuple):
+    """one descriptor-driven kernel call as a public function resolved it: the entry point and its batched op, the descriptor, the
+    streamed input as 2-D, the resolved qparams (p: scale, zero point, g_idx and the global-scale tensor, kept alive here), and the
+    output's shape and dtype.  The per-tensor functions run it (`_run`); the whole-model launches batch it."""
+    fn: str
+    op: int
+    desc: N.QuantDesc
+    src: torch.Tensor
+    p: _Problem
+    out_shape: tuple
+    out_dtype: torch.dtype
+
+
+def _call(fn: str, op: int, p: _Problem, gs, src, out_shape, out_dtype, x_dt, cd, q_dt, out_dt, qtype, bits, se=None) -> _Call:
+    p.gs = gs
+    d = _desc(p, x_dt, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, q_dt, out_dt, qtype, bits, se)
+    return _Call(fn, op, d, src, p, tuple(out_shape), out_dtype)
+
+
+def _run(c: _Call) -> torch.Tensor:
     lib = N.lib()
+    p, src, d = c.p, c.src, c.desc
     on_cpu = not src.is_cuda
     idx = _dev_index(src, p.scale)
-    gs = getattr(p, "gs", None)
     if (
         idx != _CPU
         and on_cpu
         and p.g_idx is None
-        and gs is None
-        and op not in (N.OP_QUANTIZE_PACK_FP4, N.OP_UNPACK_DEQUANTIZE_FP4)
+        and p.gs is None
+        and c.op not in (N.OP_QUANTIZE_PACK_FP4, N.OP_UNPACK_DEQUANTIZE_FP4)
         and src.numel() * src.element_size() >= _HOST_PIPELINE_MIN_BYTES
         and not p.scale.is_cuda
     ):
         # pipelined H2D / kernel / D2H on host buffers
         srcc = src.contiguous()
         zp = p.zp.contiguous() if p.zp is not None else None
-        out = torch.empty(out_shape, dtype=out_dtype, pin_memory=srcc.is_pinned())
-        host_batched(op, [(d, srcc, p.scale.contiguous(), zp, out)], idx)
+        out = torch.empty(c.out_shape, dtype=c.out_dtype, pin_memory=srcc.is_pinned())
+        host_batched(c.op, [(d, srcc, p.scale.contiguous(), zp, out)], idx)
         return out
     s_dev = _to_dev(src, idx)
     sc = _to_dev(p.scale, idx)
     zp = _to_dev(p.zp, idx)
     gi = _to_dev(p.g_idx.to(torch.int32) if p.g_idx is not None else None, idx)
-    gs_dev = _to_dev(gs, idx)   # one float32 on the device, read by the kernel (kept alive until the call returns)
+    gs_dev = _to_dev(p.gs, idx)   # one float32 on the device, read by the kernel (kept alive until the call returns)
     d.global_scale = gs_dev.data_ptr() if gs_dev is not None else None
-    out = torch.empty(out_shape, dtype=out_dtype, device=s_dev.device)
-    rc = getattr(lib, fn_name)(ctypes.byref(d), N.ptr(s_dev), N.ptr(sc), N.ptr(zp), N.ptr(gi), N.ptr(out), idx, _stream(idx))
-    N.check(rc, fn_name)
+    out = torch.empty(c.out_shape, dtype=c.out_dtype, device=s_dev.device)
+    rc = getattr(lib, c.fn)(ctypes.byref(d), N.ptr(s_dev), N.ptr(sc), N.ptr(zp), N.ptr(gi), N.ptr(out), idx, _stream(idx))
+    N.check(rc, c.fn)
     return _back(out, src)
 
 
@@ -362,31 +389,39 @@ def _like(scale, dtype):
 # --------------------------------------------------------------------------------------------
 # quantize / dequantize / fake_quantize
 # --------------------------------------------------------------------------------------------
-@torch.no_grad()
-def quantize(x, scale, zero_point, args, dtype: Optional[torch.dtype] = None, g_idx=None, global_scale=None) -> torch.Tensor:
-    """reference: quantization/lifecycle/forward.py:36-73"""
+def _quant_prologue(x, scale, global_scale, args):
+    """the checks every quantizing op runs first, in order; returns (scale, gs, effective scale dtype, qtype, bits, compute dtype)"""
     scale, gs, se = _global_scale(scale, global_scale)
     _check_float(x, "input")
     _check_float(scale, "scale")
     qtype, bits = _qparams(args)
     cd = torch.result_type(x, scale if gs is None else _like(scale, se))
-    strategy = _strategy_name(args)
-    if strategy in ("group", "tensor_group"):
-        out_dtype = dtype if dtype is not None else x.dtype  # forward_helpers.py:134,171
-    else:
-        out_dtype = dtype if dtype is not None else cd
+    return scale, gs, se, qtype, bits, cd
+
+
+def _out_dtype(args, group_dtype, other_dtype):
+    """the dtype a (fake) quantized or dequantized tensor comes back in: `group_dtype` on the group paths, `other_dtype` on the
+    others (the effective scale's dtype, or for quantize the compute dtype)"""
+    return group_dtype if _strategy_name(args) in ("group", "tensor_group") else other_dtype
+
+
+def _quantize_call(x, scale, zero_point, args, dtype=None, g_idx=None, global_scale=None) -> _Call:
+    scale, gs, se, qtype, bits, cd = _quant_prologue(x, scale, global_scale, args)
+    out_dtype = dtype if dtype is not None else _out_dtype(args, x.dtype, cd)  # forward_helpers.py:134,171
     p = _resolve(x, scale, zero_point, args, g_idx)
-    if x.device.type == "meta":
-        return torch.empty(x.shape, dtype=out_dtype, device="meta")
-    if x.numel() == 0:
-        return torch.empty(x.shape, dtype=out_dtype, device=x.device)
-    if out_dtype not in N.DT:
+    if x.device.type != "meta" and x.numel() and out_dtype not in N.DT:   # meta and empty inputs run no kernel
         raise NotImplementedError(f"quantize(dtype={out_dtype}) is not supported")
-    p.gs = gs
-    d = _desc(p, x.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, out_dtype, out_dtype, qtype, bits, se)
-    x2 = x.reshape(p.rows, p.cols)
-    out = _run("ct_quantize", N.OP_QUANTIZE, d, p, x2, (p.rows, p.cols), out_dtype)
-    return out.reshape(x.shape)
+    return _call("ct_quantize", N.OP_QUANTIZE, p, gs, x.reshape(p.rows, p.cols), (p.rows, p.cols), out_dtype,
+                 x.dtype, cd, out_dtype, out_dtype, qtype, bits, se)
+
+
+@torch.no_grad()
+def quantize(x, scale, zero_point, args, dtype: Optional[torch.dtype] = None, g_idx=None, global_scale=None) -> torch.Tensor:
+    """reference: quantization/lifecycle/forward.py:36-73"""
+    c = _quantize_call(x, scale, zero_point, args, dtype, g_idx, global_scale)
+    if x.device.type == "meta" or x.numel() == 0:
+        return torch.empty(x.shape, dtype=c.out_dtype, device=x.device)
+    return _run(c).reshape(x.shape)
 
 
 def _infer_dequant_args(x_q: torch.Tensor, scale: torch.Tensor):
@@ -409,56 +444,47 @@ def _infer_dequant_args(x_q: torch.Tensor, scale: torch.Tensor):
     )
 
 
-@torch.no_grad()
-def dequantize(x_q, scale, zero_point=None, args=None, dtype: Optional[torch.dtype] = None, g_idx=None, global_scale=None) -> torch.Tensor:
-    """reference: quantization/lifecycle/forward.py:76-145"""
+def _dequantize_call(x_q, scale, zero_point=None, args=None, dtype=None, g_idx=None, global_scale=None) -> _Call:
     if args is None:
         args = _infer_dequant_args(x_q, scale)
     if dtype is None:
         dtype = scale.dtype
     scale, gs, se = _global_scale(scale, global_scale)
     _check_float(scale, "scale")
-    strategy = _strategy_name(args)
-    # the dtype argument is honoured only on the group path (SURVEY Appendix B4)
-    out_dtype = dtype if strategy in ("group", "tensor_group") else se
+    # the dtype argument is honoured only on the group path (SURVEY Appendix B4); inferred block sizes may not cover the tensor
+    # (forward.py:118-126): the reference pads x to the block multiple, so the scale grid must be exactly ceil-div sized (_resolve)
+    out_dtype = _out_dtype(args, dtype, se)
     p = _resolve(x_q, scale, zero_point, args, g_idx)
-    if strategy == "block":
-        # inferred block sizes may not cover the tensor (forward.py:118-126); the reference pads
-        # x to the block multiple, so the scale grid must be exactly ceil-div sized (checked above)
-        pass
-    if x_q.device.type == "meta":
-        return torch.empty(x_q.shape, dtype=out_dtype, device="meta")
-    if x_q.numel() == 0:
-        return torch.empty(x_q.shape, dtype=out_dtype, device=x_q.device)
-    if x_q.dtype not in N.DT or out_dtype not in _FLOAT_DTYPES:
+    if x_q.device.type != "meta" and x_q.numel() and (x_q.dtype not in N.DT or out_dtype not in _FLOAT_DTYPES):
         raise NotImplementedError(f"dequantize from {x_q.dtype} to {out_dtype} is not supported")
-    p.gs = gs
-    d = _desc(p, None, p.scale.dtype, p.zp.dtype if p.zp is not None else None, None, x_q.dtype, out_dtype, N.Q_INT, 8, se)
-    q2 = x_q.reshape(p.rows, p.cols)
-    out = _run("ct_dequantize", N.OP_DEQUANTIZE, d, p, q2, (p.rows, p.cols), out_dtype)
-    return out.reshape(x_q.shape)
+    return _call("ct_dequantize", N.OP_DEQUANTIZE, p, gs, x_q.reshape(p.rows, p.cols), (p.rows, p.cols), out_dtype,
+                 None, None, x_q.dtype, out_dtype, N.Q_INT, 8, se)
+
+
+@torch.no_grad()
+def dequantize(x_q, scale, zero_point=None, args=None, dtype: Optional[torch.dtype] = None, g_idx=None, global_scale=None) -> torch.Tensor:
+    """reference: quantization/lifecycle/forward.py:76-145"""
+    c = _dequantize_call(x_q, scale, zero_point, args, dtype, g_idx, global_scale)
+    if x_q.device.type == "meta" or x_q.numel() == 0:
+        return torch.empty(x_q.shape, dtype=c.out_dtype, device=x_q.device)
+    return _run(c).reshape(x_q.shape)
+
+
+def _fake_quantize_call(x, scale, zero_point, args, g_idx=None, global_scale=None) -> _Call:
+    scale, gs, se, qtype, bits, cd = _quant_prologue(x, scale, global_scale, args)
+    out_dtype = _out_dtype(args, x.dtype, se)
+    p = _resolve(x, scale, zero_point, args, g_idx)
+    return _call("ct_fake_quantize", N.OP_FAKE_QUANTIZE, p, gs, x.reshape(p.rows, p.cols), (p.rows, p.cols), out_dtype,
+                 x.dtype, cd, None, out_dtype, qtype, bits, se)
 
 
 @torch.no_grad()
 def fake_quantize(x, scale, zero_point, args, g_idx=None, global_scale=None) -> torch.Tensor:
     """reference: quantization/lifecycle/forward.py:148-181"""
-    scale, gs, se = _global_scale(scale, global_scale)
-    _check_float(x, "input")
-    _check_float(scale, "scale")
-    qtype, bits = _qparams(args)
-    cd = torch.result_type(x, scale if gs is None else _like(scale, se))
-    strategy = _strategy_name(args)
-    out_dtype = x.dtype if strategy in ("group", "tensor_group") else se
-    p = _resolve(x, scale, zero_point, args, g_idx)
-    if x.device.type == "meta":
-        return torch.empty(x.shape, dtype=out_dtype, device="meta")
-    if x.numel() == 0:
-        return torch.empty(x.shape, dtype=out_dtype, device=x.device)
-    p.gs = gs
-    d = _desc(p, x.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, None, out_dtype, qtype, bits, se)
-    x2 = x.reshape(p.rows, p.cols)
-    out = _run("ct_fake_quantize", N.OP_FAKE_QUANTIZE, d, p, x2, (p.rows, p.cols), out_dtype)
-    return out.reshape(x.shape)
+    c = _fake_quantize_call(x, scale, zero_point, args, g_idx, global_scale)
+    if x.device.type == "meta" or x.numel() == 0:
+        return torch.empty(x.shape, dtype=c.out_dtype, device=x.device)
+    return _run(c).reshape(x.shape)
 
 
 def _head_job(x: torch.Tensor, scale: torch.Tensor, zp: Optional[torch.Tensor], args, out: torch.Tensor):
@@ -585,13 +611,8 @@ def dynamic_fake_quantize(x: torch.Tensor, args, global_scale: Optional[torch.Te
     out = torch.empty_like(x)
     scale = torch.empty(scale_shape, dtype=scale_dtype, device=x.device)
     zero_point = torch.empty(scale_shape, dtype=zp_dtype, device=x.device)
-    d = N.QuantDesc()
-    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, rdiv, cdiv, srs
-    d.x_dtype = d.out_dtype = N.DT[x.dtype]
-    d.scale_dtype, d.zp_dtype, d.compute_dtype, d.seff_dtype = N.DT[scale_dtype], N.DT[zp_dtype], N.DT[cd], N.DT[se]
-    d.q_dtype, d.qtype, d.num_bits = N.DT_NONE, qtype, bits
-    d.global_scale = gs.data_ptr() if gs is not None else None
-    d.aux = None
+    d = _qdesc(rows, cols, rdiv, cdiv, srs, qtype, bits, gs.data_ptr() if gs is not None else None, x_dtype=x.dtype, out_dtype=x.dtype,
+               scale_dtype=scale_dtype, zp_dtype=zp_dtype, compute_dtype=cd, seff_dtype=se)
     idx = x.get_device()
     rc = N.lib().ct_dynamic_fake_quantize(ctypes.byref(d), int(not args.symmetric), _SCALE_ROUNDING[scale_dtype_arg], N.ptr(x), N.ptr(out),
                                           N.ptr(scale), N.ptr(zero_point), idx, N.stream_ptr(idx))
@@ -742,20 +763,19 @@ def quantize_pack(x, scale, zero_point, args, g_idx=None, global_scale=None) -> 
             zp = zero_point[i] if (zero_point is not None and zero_point.ndim == x.ndim) else zero_point
             outs.append(quantize_pack(x[i], sc, zp, args, g_idx, global_scale))
         return torch.stack(outs)
-    scale, gs, se = _global_scale(scale, global_scale)
-    _check_float(x, "input")
-    _check_float(scale, "scale")
-    qtype, bits = _qparams(args)
+    c = _quantize_pack_call(x, scale, zero_point, args, g_idx, global_scale)
+    if x.device.type == "meta":
+        return torch.empty(c.out_shape, dtype=torch.int32, device="meta")
+    return _run(c)
+
+
+def _quantize_pack_call(x, scale, zero_point, args, g_idx=None, global_scale=None) -> _Call:
+    scale, gs, se, qtype, bits, cd = _quant_prologue(x, scale, global_scale, args)
     if qtype != N.Q_INT:
         raise ValueError("pack-quantized compression needs integer quantization")
-    cd = torch.result_type(x, scale if gs is None else _like(scale, se))
     p = _resolve(x, scale, zero_point, args, g_idx)
-    p.gs = gs
-    out_shape = (p.rows, math.ceil(p.cols * bits / 32))
-    if x.device.type == "meta":
-        return torch.empty(out_shape, dtype=torch.int32, device="meta")
-    d = _desc(p, x.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, torch.int8, None, qtype, bits, se)
-    return _run("ct_quantize_pack_int32", N.OP_QUANTIZE_PACK, d, p, x.reshape(p.rows, p.cols), out_shape, torch.int32)
+    return _call("ct_quantize_pack_int32", N.OP_QUANTIZE_PACK, p, gs, x.reshape(p.rows, p.cols), (p.rows, math.ceil(p.cols * bits / 32)),
+                 torch.int32, x.dtype, cd, torch.int8, None, qtype, bits, se)
 
 
 @torch.no_grad()
@@ -764,34 +784,42 @@ def unpack_dequantize(packed, scale, zero_point, num_bits: int, shape: Sequence[
     """unpack_from_int32 -> dequantize(args=None) in one pass (pack_quantized/base.py:159-166);
     the strategy is inferred from the scale shape exactly like forward.py:99-130."""
     shape = tuple(int(s) for s in shape)
-    if packed.dtype is not torch.int32:
-        raise ValueError(f"Expected {torch.int32} but got {packed.dtype}, Aborting unpack.")
-    if not 1 <= num_bits <= 8:
-        raise ValueError(f"Unpacking is only supported for num_bits in [1, 8], got {num_bits}")
     if packed.ndim > 2:
+        _check_words(packed, num_bits)
         outs = []
         for i in range(packed.shape[0]):
             sc = scale[i] if scale.ndim == packed.ndim else scale
             zp = zero_point[i] if (zero_point is not None and zero_point.ndim == packed.ndim) else zero_point
             outs.append(unpack_dequantize(packed[i], sc, zp, num_bits, shape[1:], g_idx, dtype))
         return torch.stack(outs)
+    c = _unpack_dequantize_call(packed, scale, zero_point, num_bits, shape, g_idx, dtype)
+    if packed.device.type == "meta":
+        return torch.empty(shape, dtype=c.out_dtype, device="meta")
+    return _run(c)
+
+
+def _check_words(packed, num_bits: int):
+    if packed.dtype is not torch.int32:
+        raise ValueError(f"Expected {torch.int32} but got {packed.dtype}, Aborting unpack.")
+    if not 1 <= num_bits <= 8:
+        raise ValueError(f"Unpacking is only supported for num_bits in [1, 8], got {num_bits}")
+
+
+def _unpack_dequantize_call(packed, scale, zero_point, num_bits: int, shape, g_idx=None, dtype=None) -> _Call:
+    """packed: 2-D; words past the last one `shape` needs are not read"""
+    _check_words(packed, num_bits)
     _check_float(scale, "scale")
     like = torch.empty(shape, dtype=torch.int8, device="meta")
     args = _infer_dequant_args(like, scale)
-    if dtype is None:
-        dtype = scale.dtype
-    strategy = _strategy_name(args)
-    out_dtype = dtype if strategy in ("group", "tensor_group") else scale.dtype
+    out_dtype = _out_dtype(args, dtype if dtype is not None else scale.dtype, scale.dtype)
     p = _resolve(like, scale, zero_point, args, g_idx)
     need = math.ceil(p.cols * num_bits / 32)
     if packed.shape[-1] < need:
         raise ValueError(f"packed tensor has {packed.shape[-1]} words per row, {need} needed")
     if packed.shape[-1] != need:
         packed = packed[:, :need]
-    if packed.device.type == "meta":
-        return torch.empty(shape, dtype=out_dtype, device="meta")
-    d = _desc(p, None, p.scale.dtype, p.zp.dtype if p.zp is not None else None, None, torch.int8, out_dtype, N.Q_INT, int(num_bits))
-    return _run("ct_unpack_dequantize_int32", N.OP_UNPACK_DEQUANTIZE, d, p, packed, shape, out_dtype)
+    return _call("ct_unpack_dequantize_int32", N.OP_UNPACK_DEQUANTIZE, p, None, packed, shape, out_dtype,
+                 None, None, torch.int8, out_dtype, N.Q_INT, int(num_bits))
 
 
 # --------------------------------------------------------------------------------------------
@@ -861,24 +889,23 @@ def decompress_mx_scale(scale: torch.Tensor) -> torch.Tensor:
 def quantize_pack_fp4(x, scale, zero_point, args, g_idx=None, global_scale=None) -> torch.Tensor:
     """quantize(FP4 args) -> pack_fp4_to_uint8 in one pass (compressors/nvfp4/base.py:82-90): x [R, C] float ->
     uint8 [R, C/2].  NVFP4: group 16 + global_scale; MXFP4: group 32, power-of-two scales."""
+    c = _quantize_pack_fp4_call(x, scale, zero_point, args, g_idx, global_scale)
+    if x.device.type == "meta":
+        return torch.empty(c.out_shape, dtype=torch.uint8, device="meta")
+    return _run(c)
+
+
+def _quantize_pack_fp4_call(x, scale, zero_point, args, g_idx=None, global_scale=None) -> _Call:
     if x.ndim != 2:
         raise ValueError("fp4 packing needs a 2-D weight")
     if x.shape[1] % 2 != 0:
         raise ValueError("tensor must have an even number of columns for nvfp4 compression")
-    scale, gs, se = _global_scale(scale, global_scale)
-    _check_float(x, "input")
-    _check_float(scale, "scale")
-    qtype, bits = _qparams(args)
+    scale, gs, se, qtype, bits, cd = _quant_prologue(x, scale, global_scale, args)
     if qtype != N.Q_FP4:
         raise ValueError("fp4 packing needs FLOAT quantization with num_bits == 4")
-    cd = torch.result_type(x, scale if gs is None else _like(scale, se))
     p = _resolve(x, scale, zero_point, args, g_idx)
-    p.gs = gs
-    out_shape = (p.rows, p.cols // 2)
-    if x.device.type == "meta":
-        return torch.empty(out_shape, dtype=torch.uint8, device="meta")
-    d = _desc(p, x.dtype, p.scale.dtype, p.zp.dtype if p.zp is not None else None, cd, x.dtype, None, qtype, bits, se)
-    return _run("ct_quantize_pack_fp4", N.OP_QUANTIZE_PACK_FP4, d, p, x.reshape(p.rows, p.cols), out_shape, torch.uint8)
+    return _call("ct_quantize_pack_fp4", N.OP_QUANTIZE_PACK_FP4, p, gs, x.reshape(p.rows, p.cols), (p.rows, p.cols // 2), torch.uint8,
+                 x.dtype, cd, x.dtype, None, qtype, bits, se)
 
 
 @torch.no_grad()
@@ -889,6 +916,13 @@ def unpack_dequantize_fp4(packed, scale, global_scale=None, dtype: torch.dtype =
     stored_scale="fp8" (float8_e4m3fn, NVFP4) / "e8m0" (uint8 exponents, MX), decoded in registers to `dtype`
     exactly like _decompress_scale does.
     """
+    c = _unpack_dequantize_fp4_call(packed, scale, global_scale, dtype, stored_scale)
+    if packed.device.type == "meta":
+        return torch.empty(c.out_shape, dtype=c.out_dtype, device="meta")
+    return _run(c)
+
+
+def _unpack_dequantize_fp4_call(packed, scale, global_scale=None, dtype: torch.dtype = torch.bfloat16, stored_scale=None) -> _Call:
     if packed.dtype != torch.uint8 or packed.ndim != 2:
         raise ValueError("packed fp4 weights are 2-D uint8")
     if dtype not in _FLOAT_DTYPES:
@@ -915,14 +949,12 @@ def unpack_dequantize_fp4(packed, scale, global_scale=None, dtype: torch.dtype =
         gs, se = None, base_dt
     like = torch.empty((m, n), dtype=torch.int8, device="meta")
     args = _infer_dequant_args(like, scale)
-    out_dtype = dtype if _strategy_name(args) in ("group", "tensor_group") else se
+    out_dtype = _out_dtype(args, dtype, se)
     p = _resolve(like, scale, None, args, None)
-    p.gs = gs
-    if packed.device.type == "meta":
-        return torch.empty((m, n), dtype=out_dtype, device="meta")
-    d = _desc(p, None, torch.float32, None, None, None, out_dtype, N.Q_FP4, 4, se)
-    d.scale_dtype = s_code if s_code is not None else N.DT[scale.dtype]
-    return _run("ct_unpack_dequantize_fp4", N.OP_UNPACK_DEQUANTIZE_FP4, d, p, packed, (m, n), out_dtype)
+    c = _call("ct_unpack_dequantize_fp4", N.OP_UNPACK_DEQUANTIZE_FP4, p, gs, packed, (m, n), out_dtype, None, None, None, out_dtype,
+              N.Q_FP4, 4, se)
+    c.desc.scale_dtype = s_code if s_code is not None else N.DT[scale.dtype]
+    return c
 
 
 # --------------------------------------------------------------------------------------------
@@ -932,6 +964,13 @@ def unpack_dequantize_fp4(packed, scale, global_scale=None, dtype: torch.dtype =
 def dequantize_block_fp8(weight: torch.Tensor, scale_inv: torch.Tensor, block_size: Sequence[int], dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
     """(weight.to(float32) * scale_inv.to(float32) per block).to(dtype): entrypoints/convert/converters/fp8block_dequantizer.py:111-158.
     weight float8_e4m3fn [R, C], scale_inv [ceil(R/bh), ceil(C/bw)]; one kernel, no padded copy."""
+    c = _dequantize_block_fp8_call(weight, scale_inv, block_size, dtype)
+    if weight.device.type == "meta" or weight.numel() == 0:
+        return torch.empty(weight.shape, dtype=dtype, device=weight.device)
+    return _run(c)
+
+
+def _dequantize_block_fp8_call(weight, scale_inv, block_size, dtype=torch.bfloat16) -> _Call:
     from types import SimpleNamespace
 
     if weight.ndim != 2 or weight.dtype != torch.float8_e4m3fn:
@@ -941,12 +980,9 @@ def dequantize_block_fp8(weight: torch.Tensor, scale_inv: torch.Tensor, block_si
     scale = scale_inv.to(torch.float32)   # qparam-sized; float32 already in the checkpoints this converter targets
     args = SimpleNamespace(strategy="block", group_size=None, block_structure=[int(block_size[0]), int(block_size[1])])
     p = _resolve(weight, scale, None, args, None)
-    if weight.device.type == "meta":
-        return torch.empty(weight.shape, dtype=dtype, device="meta")
-    if weight.numel() == 0:
-        return torch.empty(weight.shape, dtype=dtype, device=weight.device)
-    d = _desc(p, None, torch.float32, None, None, weight.dtype, dtype, N.Q_INT, 8, torch.float32)
-    return _run("ct_dequantize", N.OP_DEQUANTIZE, d, p, weight, tuple(weight.shape), dtype)
+    # the block dequantization of `dequantize`, but in the requested dtype, which `dequantize` honours on the group path only
+    return _call("ct_dequantize", N.OP_DEQUANTIZE, p, None, weight, weight.shape, dtype, None, None, weight.dtype, dtype, N.Q_INT, 8,
+                 torch.float32)
 
 
 def _awq(fn_name: str, src: torch.Tensor, out_shape, rows: int, n_out: int) -> torch.Tensor:
@@ -976,15 +1012,9 @@ def _tensor_observer_ok(xd: torch.Tensor) -> bool:
 
 
 def _tensor_desc(xd: torch.Tensor, qtype: int, bits: int, q_dt=None, asym: bool = False) -> N.QuantDesc:
-    d = N.QuantDesc()
     cols = xd.shape[-1] if xd.ndim >= 1 else 1
-    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = xd.numel() // max(cols, 1), cols, N.INF, N.INF, 0
-    d.x_dtype = d.scale_dtype = d.compute_dtype = N.DT[xd.dtype]
-    d.zp_dtype = N.DT[torch.int8] if asym else N.DT_NONE
-    d.q_dtype = N.DT[q_dt] if q_dt is not None else N.DT_NONE
-    d.out_dtype, d.qtype, d.num_bits = N.DT_NONE, qtype, bits
-    d.global_scale, d.seff_dtype, d.aux = None, N.DT_NONE, None
-    return d
+    return _qdesc(xd.numel() // max(cols, 1), cols, N.INF, N.INF, 0, qtype, bits, x_dtype=xd.dtype, scale_dtype=xd.dtype,
+                  compute_dtype=xd.dtype, zp_dtype=torch.int8 if asym else None, q_dtype=q_dt)
 
 
 @torch.no_grad()
@@ -1027,8 +1057,6 @@ def observe_quantize_pack(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Te
     -> quantize(dtype=int8) -> pack_to_int32, bit for bit.  The fused kernel covers group quantization of
     bf16 / fp16 weights with group_size in {32, 64, 128, 256} and 4- or 8-bit codes; every other case runs
     the same three steps as separate GPU ops."""
-    from .quantization.utils.helpers import calculate_qparams  # host-side qparam rule (tiny tensors)
-
     qtype, bits = _qparams(args)
     strategy = _strategy_name(args)
     symmetric = bool(getattr(args, "symmetric", True))
@@ -1046,15 +1074,20 @@ def observe_quantize_pack(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Te
         scale = torch.empty((rows, ng), dtype=x.dtype, device=xd.device)
         zp = None if symmetric else torch.empty((rows, ng), dtype=torch.int8, device=xd.device)
         packed = torch.empty((rows, cols * bits // 32), dtype=torch.int32, device=xd.device)
-        d = N.QuantDesc()
-        d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, 1, group, ng
-        d.x_dtype = d.scale_dtype = d.compute_dtype = N.DT[x.dtype]
-        d.zp_dtype = N.DT_NONE if symmetric else N.DT[torch.int8]
-        d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT[torch.int8], N.DT_NONE, qtype, bits
+        d = _qdesc(rows, cols, 1, group, ng, qtype, bits, x_dtype=x.dtype, scale_dtype=x.dtype, compute_dtype=x.dtype,
+                   zp_dtype=None if symmetric else torch.int8, q_dtype=torch.int8)
         rc = N.lib().ct_observe_quantize_pack_int32(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(packed), idx, N.stream_ptr(idx))
         N.check(rc, "observe_quantize_pack")
         return _back(packed, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
-    # unfused: observer with torch reductions on the device, then the fused quantize+pack kernel
+    return _observe_unfused("observe_quantize_pack", x, xd, args, group, True, torch.int32)
+
+
+def _observe_unfused(who: str, x, xd, args, group: int, pack: bool, qdt):
+    """the observer with torch reductions on the device (min / max per group, channel or tensor -> calculate_qparams), then the
+    quantize (pack: quantize + pack) kernel; returns (codes, scale, zero point or None) where x lives"""
+    from .quantization.utils.helpers import calculate_qparams
+
+    strategy = _strategy_name(args)
     if strategy == "group":
         xr = xd.unflatten(-1, (-1, group))
         mn, mx = xr.amin(-1), xr.amax(-1)
@@ -1063,11 +1096,11 @@ def observe_quantize_pack(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Te
     elif strategy == "tensor":
         mn, mx = (t.reshape(1) for t in torch.aminmax(xd))
     else:
-        raise NotImplementedError(f"observe_quantize_pack does not support strategy {strategy}")
+        raise NotImplementedError(f"{who} does not support strategy {strategy}")
     scale, zp = calculate_qparams(mn, mx, args)
-    zp = None if symmetric else zp
-    packed = quantize_pack(xd, scale, zp, args)
-    return _back(packed, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+    zp = None if bool(getattr(args, "symmetric", True)) else zp
+    out = quantize_pack(xd, scale, zp, args) if pack else quantize(xd, scale, zp, args, dtype=qdt)
+    return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
 
 
 @torch.no_grad()
@@ -1101,11 +1134,7 @@ def observe_quantize_pack_nvfp4(x: torch.Tensor, args, global_scale: Optional[to
     if x.dtype in (torch.bfloat16, torch.float16) and cols % 32 == 0 and rows > 0:
         scale = torch.empty((rows, cols // 16), dtype=torch.float8_e4m3fn, device=xd.device)
         packed = torch.empty((rows, cols // 2), dtype=torch.uint8, device=xd.device)
-        d = N.QuantDesc()
-        d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, 1, 16, cols // 16
-        d.x_dtype, d.scale_dtype, d.compute_dtype = N.DT[x.dtype], N.DT[torch.float8_e4m3fn], N.DT[torch.float32]
-        d.zp_dtype, d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT_NONE, N.DT[x.dtype], N.DT_NONE, N.Q_FP4, 4
-        d.global_scale, d.seff_dtype = gs.data_ptr(), N.DT[torch.float32]
+        d = _nvfp4_observe_desc(rows, cols, x.dtype, gs.data_ptr())
         rc = N.lib().ct_observe_quantize_pack_nvfp4(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(packed), idx, N.stream_ptr(idx))
         N.check(rc, "observe_quantize_pack_nvfp4")
         return _back(packed, x), _back(scale, x), _back(gs, x)
@@ -1115,26 +1144,23 @@ def observe_quantize_pack_nvfp4(x: torch.Tensor, args, global_scale: Optional[to
     return _back(packed, x), _back(scale.to(torch.float8_e4m3fn), x), _back(gs, x)
 
 
+def _nvfp4_observe_desc(rows: int, cols: int, x_dtype: torch.dtype, global_scale) -> N.QuantDesc:
+    """descriptor of `ct_observe_quantize_pack_nvfp4` / batched op OP_OBSERVE_QUANTIZE_PACK_FP4: float8_e4m3fn scales written per
+    group of 16, a float32 global scale at `global_scale`"""
+    return _qdesc(rows, cols, 1, 16, cols // 16, N.Q_FP4, 4, global_scale, x_dtype=x_dtype, scale_dtype=torch.float8_e4m3fn,
+                  compute_dtype=torch.float32, q_dtype=x_dtype, seff_dtype=torch.float32)
+
+
 def _block_desc(rows: int, cols: int, bh: int, bw: int, x_dtype: torch.dtype) -> N.QuantDesc:
     """descriptor of `ct_observe_quantize_block` / batched op OP_OBSERVE_QUANTIZE_BLOCK for an fp8 weight [rows, cols] in blocks [bh, bw]"""
-    d = N.QuantDesc()
-    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, bh, bw, -(-cols // bw)
-    d.x_dtype = d.scale_dtype = d.compute_dtype = N.DT[x_dtype]
-    d.zp_dtype, d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT_NONE, N.DT[torch.float8_e4m3fn], N.DT_NONE, N.Q_FLOAT, 8
-    d.global_scale, d.seff_dtype, d.aux = None, N.DT_NONE, None
-    return d
+    return _qdesc(rows, cols, bh, bw, -(-cols // bw), N.Q_FLOAT, 8, x_dtype=x_dtype, scale_dtype=x_dtype, compute_dtype=x_dtype,
+                  q_dtype=torch.float8_e4m3fn)
 
 
 def _mx_desc(rows: int, cols: int, bits: int, x_dtype: torch.dtype) -> N.QuantDesc:
     """descriptor of `ct_observe_quantize_mx` / batched op OP_OBSERVE_QUANTIZE_MX: MXFP4 (bits 4) or MXFP8 (bits 8), groups of 32"""
-    d = N.QuantDesc()
-    d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, 1, 32, cols // 32
-    d.x_dtype = d.compute_dtype = N.DT[x_dtype]
-    d.scale_dtype, d.zp_dtype, d.out_dtype = N.DT_E8M0, N.DT_NONE, N.DT_NONE
-    d.qtype, d.num_bits = (N.Q_FP4, 4) if bits == 4 else (N.Q_FLOAT, 8)
-    d.q_dtype = N.DT[torch.uint8] if bits == 4 else N.DT[torch.float8_e4m3fn]
-    d.global_scale, d.seff_dtype, d.aux = None, N.DT_NONE, None
-    return d
+    qtype, bits, q_dt = (N.Q_FP4, 4, torch.uint8) if bits == 4 else (N.Q_FLOAT, 8, torch.float8_e4m3fn)
+    return _qdesc(rows, cols, 1, 32, cols // 32, qtype, bits, x_dtype=x_dtype, compute_dtype=x_dtype, scale_dtype=N.DT_E8M0, q_dtype=q_dt)
 
 
 def _aligned(*tensors: torch.Tensor) -> bool:
@@ -1237,8 +1263,6 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
       BLOCK (FP8_BLOCK)          : `ct_observe_quantize_block` -- one CTA per block: min / max, calculate_qparams, fp8 codes; returns
                                    (float8_e4m3fn [R, C], scale in x.dtype [ceil(R / bh), ceil(C / bw)], None)
     Everything else runs the observer with torch reductions on the device and then the quantize kernel."""
-    from .quantization.utils.helpers import calculate_qparams
-
     qtype, bits = _qparams(args)
     strategy = _strategy_name(args)
     symmetric = bool(getattr(args, "symmetric", True))
@@ -1260,11 +1284,8 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
         scale = torch.empty((rows, 1), dtype=x.dtype, device=xd.device)
         zp = None if symmetric else torch.empty((rows, 1), dtype=torch.int8, device=xd.device)
         out = torch.empty((rows, cols * bits // 32) if pack else (rows, cols), dtype=qdt, device=xd.device)
-        d = N.QuantDesc()
-        d.rows, d.cols, d.rdiv, d.cdiv, d.s_row_stride = rows, cols, 1, N.INF, 1
-        d.x_dtype = d.scale_dtype = d.compute_dtype = N.DT[x.dtype]
-        d.zp_dtype = N.DT_NONE if symmetric else N.DT[torch.int8]
-        d.q_dtype, d.out_dtype, d.qtype, d.num_bits = N.DT[qdt], N.DT_NONE, qtype, bits
+        d = _qdesc(rows, cols, 1, N.INF, 1, qtype, bits, x_dtype=x.dtype, scale_dtype=x.dtype, compute_dtype=x.dtype,
+                   zp_dtype=None if symmetric else torch.int8, q_dtype=qdt)
         rc = N.lib().ct_observe_quantize_channel(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(out), idx, N.stream_ptr(idx))
         if rc != N.CT_E_UNSUPPORTED:   # declined (a row wider than one cluster holds): the unfused path below
             N.check(rc, "observe_quantize")
@@ -1279,28 +1300,13 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
         rc = N.lib().ct_observe_quantize_tensor(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(out), idx, N.stream_ptr(idx))
         N.check(rc, "observe_quantize")
         return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
-    if strategy == "group":
-        group = int(getattr(args, "group_size"))
-        xr = xd.unflatten(-1, (-1, group))
-        mn, mx = xr.amin(-1), xr.amax(-1)
-    elif strategy == "channel":
-        mn, mx = xd.amin(-1, keepdim=True), xd.amax(-1, keepdim=True)
-    elif strategy == "tensor":
-        mn, mx = (t.reshape(1) for t in torch.aminmax(xd))
-    else:
-        raise NotImplementedError(f"observe_quantize does not support strategy {strategy}")
-    scale, zp = calculate_qparams(mn, mx, args)
-    zp = None if symmetric else zp
-    out = quantize_pack(xd, scale, zp, args) if pack else quantize(xd, scale, zp, args, dtype=qdt)
-    return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+    group = int(getattr(args, "group_size")) if strategy == "group" else 0
+    return _observe_unfused("observe_quantize", x, xd, args, group, pack, qdt)
 
 
 # --------------------------------------------------------------------------------------------
 # multi-tensor launch (the module loop of ModelCompressor.compress_model in one kernel)
 # --------------------------------------------------------------------------------------------
-_DT_SIZE = {0: 4, 1: 2, 2: 2, 3: 1, 4: 1, 5: 4, 6: 1, 7: 8, 8: 1}     # bytes per element of each ct_dtype_t
-
-
 def _scale_count(d: N.QuantDesc) -> int:
     """elements of the scale / zero-point tensor that the addressing  sidx = (r / rdiv) * s_row_stride + c / cdiv  can reach"""
     row_scaled = d.rdiv != N.INF
@@ -1324,31 +1330,31 @@ def _validate_problem(op: int, i: int, prob, on_cuda: Optional[int]) -> None:
     words = rows * (-(-cols * bits // 32)) if bits > 0 else 0
     # (input elements, input bytes/elem, output elements, output bytes/elem); None = not checked for this op
     if op in (N.OP_QUANTIZE_PACK, N.OP_OBSERVE_QUANTIZE_PACK):
-        want = (n, _DT_SIZE.get(d.x_dtype), words, 4)
+        want = (n, N.DT_SIZE.get(d.x_dtype), words, 4)
     elif op == N.OP_UNPACK_DEQUANTIZE:
-        want = (words, 4, n, _DT_SIZE.get(d.out_dtype))
+        want = (words, 4, n, N.DT_SIZE.get(d.out_dtype))
     elif op == N.OP_QUANTIZE:
-        want = (n, _DT_SIZE.get(d.x_dtype), n, _DT_SIZE.get(d.q_dtype))
+        want = (n, N.DT_SIZE.get(d.x_dtype), n, N.DT_SIZE.get(d.q_dtype))
     elif op == N.OP_DEQUANTIZE:
-        want = (n, _DT_SIZE.get(d.q_dtype), n, _DT_SIZE.get(d.out_dtype))
+        want = (n, N.DT_SIZE.get(d.q_dtype), n, N.DT_SIZE.get(d.out_dtype))
     elif op == N.OP_FAKE_QUANTIZE:
-        want = (n, _DT_SIZE.get(d.x_dtype), n, _DT_SIZE.get(d.out_dtype))
+        want = (n, N.DT_SIZE.get(d.x_dtype), n, N.DT_SIZE.get(d.out_dtype))
     elif op == N.OP_PACK_INT32:
         want = (n, 1, words, 4)
     elif op == N.OP_UNPACK_INT32:
         want = (words, 4, n, 1)
     elif op in (N.OP_QUANTIZE_PACK_FP4, N.OP_OBSERVE_QUANTIZE_PACK_FP4):
-        want = (n, _DT_SIZE.get(d.x_dtype), n // 2, 1)
+        want = (n, N.DT_SIZE.get(d.x_dtype), n // 2, 1)
     elif op == N.OP_UNPACK_DEQUANTIZE_FP4:
-        want = (n // 2, 1, n, _DT_SIZE.get(d.out_dtype))
+        want = (n // 2, 1, n, N.DT_SIZE.get(d.out_dtype))
     elif op == N.OP_OBSERVE_QUANTIZE_BLOCK:
-        want = (n, _DT_SIZE.get(d.x_dtype), n, 1)
+        want = (n, N.DT_SIZE.get(d.x_dtype), n, 1)
     elif op == N.OP_OBSERVE_QUANTIZE_MX:
-        want = (n, _DT_SIZE.get(d.x_dtype), n // 2 if d.qtype == N.Q_FP4 else n, 1)
+        want = (n, N.DT_SIZE.get(d.x_dtype), n // 2 if d.qtype == N.Q_FP4 else n, 1)
     elif op == N.OP_SPARSE24_QUANTIZE_PACK:          # kept codes [rows, cols/2] as a 4-bit stream; the bitmask (d.aux) is the caller's business
-        want = (n, _DT_SIZE.get(d.x_dtype), rows * (-(-(cols // 2) * bits // 32)), 4)
+        want = (n, N.DT_SIZE.get(d.x_dtype), rows * (-(-(cols // 2) * bits // 32)), 4)
     elif op == N.OP_SPARSE24_UNPACK_DEQUANTIZE:
-        want = (rows * (-(-(cols // 2) * bits // 32)), 4, n, _DT_SIZE.get(d.out_dtype))
+        want = (rows * (-(-(cols // 2) * bits // 32)), 4, n, N.DT_SIZE.get(d.out_dtype))
     else:
         bad(f"unknown op {op}")
     for what, t, numel, size in (("input", tin, want[0], want[1]), ("output", out, want[2], want[3])):
@@ -1362,13 +1368,13 @@ def _validate_problem(op: int, i: int, prob, on_cuda: Optional[int]) -> None:
     if op not in (N.OP_PACK_INT32, N.OP_UNPACK_INT32):
         if sc is None:
             bad("scale tensor is missing")
-        ssize = _DT_SIZE.get(d.scale_dtype)
+        ssize = N.DT_SIZE.get(d.scale_dtype)
         need = _scale_count(d)
         if ssize is None or sc.element_size() != ssize or sc.numel() < need:
             bad(f"scale holds {sc.numel()} elements of {sc.element_size()} bytes, the descriptor addresses {need} of {ssize}")
         tensors.append(("scale", sc))
         if zp is not None:
-            zsize = _DT_SIZE.get(d.zp_dtype)
+            zsize = N.DT_SIZE.get(d.zp_dtype)
             if zsize is None or zp.element_size() != zsize or zp.numel() < need:
                 bad(f"zero point holds {zp.numel()} elements of {zp.element_size()} bytes, the descriptor addresses {need} of {zsize}")
             tensors.append(("zero point", zp))

@@ -247,31 +247,26 @@ def oracle_kw(args) -> dict:
 
 
 def quant_desc(op: str, x, scale, zp, args):
-    """(desc, expected output) of one quantize-family op, the descriptor built the way ops.py builds it"""
-    qtype, bits = ops._qparams(args)
-    p = ops._resolve(x, scale, zp, args, None)
-    zdt = zp.dtype if zp is not None else None
-    cd = torch.result_type(x, scale)
+    """(desc, expected output) of one quantize-family op, the descriptor built by the op's own recipe in ops.py"""
+    bits = int(args.num_bits)
     kw = oracle_kw(args)
     okw = dict(kw, num_bits=bits, qtype=args.type)
     q_dt = torch.float8_e4m3fn if args.type == "float" else torch.int8
     if op == "quantize":
-        d = ops._desc(p, x.dtype, scale.dtype, zdt, cd, q_dt, q_dt, qtype, bits)
-        return d, oracle.quantize(x, scale, zp, dtype=q_dt, **okw)
+        return ops._quantize_call(x, scale, zp, args, dtype=q_dt).desc, oracle.quantize(x, scale, zp, dtype=q_dt, **okw)
     codes = oracle.quantize(x, scale, zp, dtype=torch.int8, **okw)
     if op == "dequantize":
-        out_dt = scale.dtype
-        d = ops._desc(p, None, scale.dtype, zdt, None, torch.int8, out_dt, N.Q_INT, 8)
-        return d, oracle.dequantize(codes, scale, zp, dtype=out_dt, **kw).to(out_dt)
+        c = ops._dequantize_call(codes, scale, zp, args)
+        return c.desc, oracle.dequantize(codes, scale, zp, dtype=c.out_dtype, **kw).to(c.out_dtype)
     if op == "fake_quantize":
-        out_dt = x.dtype if args.strategy == "group" else scale.dtype
-        d = ops._desc(p, x.dtype, scale.dtype, zdt, cd, None, out_dt, qtype, bits)
-        return d, oracle.fake_quantize(x, scale, zp, **okw)
+        return ops._fake_quantize_call(x, scale, zp, args).desc, oracle.fake_quantize(x, scale, zp, **okw)
     if op == "quantize_pack":
-        d = ops._desc(p, x.dtype, scale.dtype, zdt, cd, torch.int8, None, qtype, bits)
-        return d, oracle.pack_to_int32(codes, bits)
+        return ops._quantize_pack_call(x, scale, zp, args).desc, oracle.pack_to_int32(codes, bits)
     assert op == "unpack_dequantize"
-    d = ops._desc(p, None, scale.dtype, zdt, None, torch.int8, scale.dtype, N.Q_INT, bits)
+    # unpack_dequantize infers its strategy from the scale shape, which cannot name every block layout these problems use:
+    # the same descriptor, with the problem's own args
+    p = ops._resolve(x, scale, zp, args, None)
+    d = ops._desc(p, None, scale.dtype, zp.dtype if zp is not None else None, None, torch.int8, scale.dtype, N.Q_INT, bits)
     return d, oracle.dequantize(codes, scale, zp, dtype=scale.dtype, **kw).to(scale.dtype)
 
 

@@ -31,28 +31,24 @@ def build_problems(layers: int):
     keep = []
     sc_out = [torch.empty_like(s) for s in scs]
     for w, sc, o, b, s, q, so in zip(ws, scs, outs, back, s8, q8, sc_out):
-        p = ops._resolve(w, sc, None, qa, None)
-        P["observe_qp"].append((ops._desc(p, w.dtype, sc.dtype, None, torch.bfloat16, torch.int8, None, N.Q_INT, 4), w, so, None, o))
-        P["quantpack"].append((ops._desc(p, w.dtype, sc.dtype, None, torch.bfloat16, torch.int8, None, N.Q_INT, 4), w, sc, None, o))
-        P["unpackdeq"].append((ops._desc(p, None, sc.dtype, None, None, torch.int8, torch.bfloat16, N.Q_INT, 4), o, sc, None, b))
-        P["fake_w4"].append((ops._desc(p, w.dtype, sc.dtype, None, torch.bfloat16, None, torch.bfloat16, N.Q_INT, 4), w, sc, None, b))
-        p8 = ops._resolve(w, s, None, f8, None)
-        P["fp8_q"].append((ops._desc(p8, w.dtype, s.dtype, None, torch.bfloat16, torch.float8_e4m3fn, None, N.Q_FLOAT, 8), w, s, None, q))
+        qp = ops._quantize_pack_call(w, sc, None, qa).desc
+        P["observe_qp"].append((qp, w, so, None, o))      # the observer writes the scale: same descriptor, scale as an output
+        P["quantpack"].append((qp, w, sc, None, o))
+        P["unpackdeq"].append((ops._unpack_dequantize_call(o, sc, None, 4, w.shape).desc, o, sc, None, b))
+        P["fake_w4"].append((ops._fake_quantize_call(w, sc, None, qa).desc, w, sc, None, b))
+        P["fp8_q"].append((ops._quantize_call(w, s, None, f8, dtype=torch.float8_e4m3fn).desc, w, s, None, q))
         g = (448.0 * 6.0 / w.abs().max().float()).reshape(1)
         s8n = (w.unflatten(-1, (-1, 16)).abs().amax(-1).float() / 6.0 * g).clamp(2.0 ** -9, 448.0).to(torch.float8_e4m3fn)
         sbn = s8n.to(torch.bfloat16)
         nib = torch.empty(w.shape[0], w.shape[1] // 2, dtype=torch.uint8, device=dev)
-        pn = ops._resolve(w, sbn, None, nv, None)
-        dn = ops._desc(pn, w.dtype, sbn.dtype, None, torch.float32, w.dtype, None, N.Q_FP4, 4, torch.float32)
-        dn.global_scale = g.data_ptr()
-        du = ops._desc(pn, None, torch.float32, None, None, None, torch.bfloat16, N.Q_FP4, 4, torch.float32)
-        du.scale_dtype = N.DT[torch.float8_e4m3fn]
-        du.global_scale = g.data_ptr()
+        dn = ops._quantize_pack_fp4_call(w, sbn, None, nv, global_scale=g).desc
+        du = ops._unpack_dequantize_fp4_call(nib, s8n, g, torch.bfloat16, stored_scale="fp8").desc
+        dn.global_scale = du.global_scale = g.data_ptr()   # the recipes leave the device pointer to the launch
         keep.append(g)
         P["nvfp4_qp"].append((dn, w, sbn, None, nib))
-        P.setdefault("nvfp4_observe_qp", []).append((dn, w, torch.empty_like(s8n), None, nib))
+        P.setdefault("nvfp4_observe_qp", []).append((ops._nvfp4_observe_desc(*w.shape, w.dtype, g.data_ptr()), w, torch.empty_like(s8n), None, nib))
         P["nvfp4_ud"].append((du, nib, s8n, None, b))
-        P["fp8_dq"].append((ops._desc(p8, None, s.dtype, None, None, torch.float8_e4m3fn, torch.bfloat16, N.Q_INT, 8), q, s, None, b))
+        P["fp8_dq"].append((ops._dequantize_call(q, s, None, f8).desc, q, s, None, b))
     OPS = {"quantpack": (N.OP_QUANTIZE_PACK, 2.515625), "unpackdeq": (N.OP_UNPACK_DEQUANTIZE, 2.515625),
            "observe_qp": (N.OP_OBSERVE_QUANTIZE_PACK, 2.515625), "fp8_q": (N.OP_QUANTIZE, 3.0), "fp8_dq": (N.OP_DEQUANTIZE, 3.0), "fake_w4": (N.OP_FAKE_QUANTIZE, 4.0 + 2 / 128),
            "nvfp4_qp": (N.OP_QUANTIZE_PACK_FP4, 2 + 2 / 16 + 0.5), "nvfp4_observe_qp": (N.OP_OBSERVE_QUANTIZE_PACK_FP4, 2 + 1 / 16 + 0.5), "nvfp4_ud": (N.OP_UNPACK_DEQUANTIZE_FP4, 0.5 + 1 / 16 + 2)}

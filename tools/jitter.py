@@ -39,15 +39,10 @@ def main():
     jobs["int4_pack"] = (N.OP_PACK_INT32, [(d, c, None, None, o) for d, c, o in zip(descs, codes, pk)], nel * 1.5)
     jobs["int4_unpack"] = (N.OP_UNPACK_INT32, [(d, o, None, None, c) for d, c, o in zip(descs, codes, pk)], nel * 1.5)
     # checkpoint converters: FP8 128x128-block dequantize (DeepSeek-style shapes) and the AutoAWQ nibble transpose
-    from types import SimpleNamespace
-    blk = SimpleNamespace(strategy="block", group_size=None, block_structure=[128, 128])
     fw = [torch.randn(7168, 4096, device=dev).to(torch.float8_e4m3fn) for _ in range(8)]
     fs = [torch.rand(56, 32, device=dev) * 0.01 + 1e-4 for _ in fw]
     fo = [torch.empty(w.shape, dtype=torch.bfloat16, device=dev) for w in fw]
-    fprobs = []
-    for w, sc, o in zip(fw, fs, fo):
-        p = ops._resolve(w, sc, None, blk, None)
-        fprobs.append((ops._desc(p, None, torch.float32, None, None, w.dtype, torch.bfloat16, N.Q_INT, 8, torch.float32), w, sc, None, o))
+    fprobs = [(ops._dequantize_block_fp8_call(w, sc, (128, 128)).desc, w, sc, None, o) for w, sc, o in zip(fw, fs, fo)]
     jobs["fp8_block_dq"] = (N.OP_DEQUANTIZE, fprobs, sum(w.numel() for w in fw) * 3.0)
     awq_q = torch.randint(-2 ** 31, 2 ** 31 - 1, (14336, 4096 // 8), device=dev, dtype=torch.int64).to(torch.int32)
     extra_fns = {"awq_repack": (lambda: ops.awq_repack(awq_q), 14336 * 4096 * 1.0)}

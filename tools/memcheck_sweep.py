@@ -124,6 +124,13 @@ def converter_family(rows, cols):
         ops.awq_repack_zeros(q[: max(1, rows // 128)])
 
 
+def _dense_unpack_desc(scale, bits, shape):
+    """the unpack + dequantize descriptor of a dense [rows, cols] output: the 2:4 stream holds half the words, so the recipe is
+    given a placeholder of the dense packed width (it reads only its shape)"""
+    words = torch.empty((shape[0], -(-shape[1] * bits // 32)), dtype=torch.int32, device="meta")
+    return ops._unpack_dequantize_call(words, scale, None, bits, shape).desc
+
+
 def batched_family(dt):
     """the multi-tensor persistent launch (what ModelCompressor.compress_model uses) with tensors of unequal size"""
     a = qa(num_bits=4, type="int", strategy="group", group_size=128)
@@ -132,8 +139,7 @@ def batched_family(dt):
         x = torch.randn(rows, cols, device=DEV).to(dt)
         s = scale_for(x, (rows, cols // 128), 7.5)
         out = torch.empty(rows, cols // 8, dtype=torch.int32, device=DEV)
-        p = ops._resolve(x, s, None, a, None)
-        probs.append((ops._desc(p, dt, dt, None, dt, torch.int8, None, N.Q_INT, 4), x, s, None, out))
+        probs.append((ops._quantize_pack_call(x, s, None, a).desc, x, s, None, out))
     ops.batched(N.OP_QUANTIZE_PACK, probs, 0)
     # round 2: the fused 2:4 + int4 ops as multi-tensor launches (bitmask in desc.aux)
     c24, d24, keep = [], [], []
@@ -144,9 +150,7 @@ def batched_family(dt):
         pk = torch.empty(rows, cols // 16, dtype=torch.int32, device=DEV)
         bm = torch.empty(rows, cols // 8, dtype=torch.uint8, device=DEV)
         bk = torch.empty_like(x)
-        p = ops._resolve(x, s, None, a, None)
-        d1 = ops._desc(p, dt, dt, None, dt, torch.int8, None, N.Q_INT, 4)
-        d2 = ops._desc(p, None, dt, None, None, torch.int8, dt, N.Q_INT, 4)
+        d1, d2 = ops._quantize_pack_call(x, s, None, a).desc, _dense_unpack_desc(s, 4, (rows, cols))
         d1.aux = d2.aux = bm.data_ptr()
         c24.append((d1, x, s, None, pk)); d24.append((d2, pk, s, None, bk)); keep.append(bm)
     ops.batched(N.OP_SPARSE24_QUANTIZE_PACK, c24, 0)
