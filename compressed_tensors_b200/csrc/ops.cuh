@@ -17,11 +17,11 @@ struct F32 {
 };
 
 enum QKind { QI_NARROW = 0, QI_WIDE = 1, QF8 = 2 };
-// rounding kind of fake_quantize on compute dtype p_dt: the packed magic-number rounding in T (QI_NARROW) covers codes of up to 7 bits
-// in bf16 and 8 in fp16; wider codes and fp32 round through rintf (QI_WIDE)
+// rounding kind of fake_quantize on compute dtype p_dt: the packed magic-number rounding in T (QI_NARROW) covers codes of up to
+// P::MAGIC_MAX_BITS bits (7 in bf16, 8 in fp16); wider codes and fp32 round through rintf (QI_WIDE)
 inline int fake_kind(int p_dt, int qtype, int bits) {
     if (qtype == CT_Q_FLOAT) return QF8;
-    return (p_dt == CT_F32 || bits > (p_dt == CT_BF16 ? 7 : 8)) ? QI_WIDE : QI_NARROW;
+    return (p_dt == CT_F32 || bits > (p_dt == CT_BF16 ? BF16::MAGIC_MAX_BITS : F16::MAGIC_MAX_BITS)) ? QI_WIDE : QI_NARROW;
 }
 
 template <class P> struct ElemBytes { static constexpr int v = 2; };
