@@ -73,6 +73,24 @@ class QuantDesc(ctypes.Structure):
     ]
 
 
+MSE_MAX_STEPS = 64
+
+
+class MseBlock(ctypes.Structure):
+    """mirror of `struct ct_mse_block` (include/ct_b200.h): the MSE observer's search, pointed to by ct_quant_desc.aux"""
+
+    _fields_ = [
+        ("shrink", ctypes.c_float * MSE_MAX_STEPS),
+        ("steps", ctypes.c_int32),
+        ("patience", ctypes.c_int32),
+        ("norm", ctypes.c_float),
+        ("_reserved", ctypes.c_int32),
+        ("any", ctypes.c_uint64),
+        ("masks", ctypes.c_void_p),
+        ("errors", ctypes.c_void_p),
+    ]
+
+
 class HeadJob(ctypes.Structure):
     """mirror of `struct ct_head_job` (include/ct_b200.h)"""
 

@@ -146,7 +146,7 @@ static Plan plan_one(int op, const ct_quant_desc& d, const void* in, const void*
         if (d.x_dtype != d.scale_dtype || d.x_dtype != d.compute_dtype || (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16)) return {};
         if (is_inf(D) || D != d.cdiv || D % 32 != 0) return {};
         p_dt = d.x_dtype; in_bytes_per_chunk = 16;
-        k = observe_kernel(p_dt, d.num_bits, zp != nullptr, (int)(D / 32));
+        k = observe_kernel(p_dt, d.num_bits, zp != nullptr, (int)(D / 32), d.aux != nullptr);
         break;
     }
     case CT_OP_UNPACK_DEQUANTIZE:
@@ -185,7 +185,8 @@ static Plan plan_one(int op, const ct_quant_desc& d, const void* in, const void*
     }
     // a partial last tile must still be a multiple of 16 bytes for the bulk copy
     if (((n / 8) * in_bytes_per_chunk) % 16 != 0) return {};
-    return fast_plan(k, make_common(p_dt, d.qtype, d.num_bits), in, scale, zp, out, nullptr, n, 8, D, two_d ? &d : nullptr);
+    return fast_plan(k, make_common(p_dt, d.qtype, d.num_bits), in, scale, zp, out, op == CT_OP_OBSERVE_QUANTIZE_PACK ? d.aux : nullptr, n, 8, D,
+                     two_d ? &d : nullptr);
 }
 
 // FP4 fused ops as streaming jobs (fast_fp4.cu).  Both need GROUP strategy with full rows of scales and no g_idx.
@@ -205,7 +206,8 @@ static Plan plan_fp4(int op, const ct_quant_desc& d, const void* in, const void*
         if ((d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) || d.cols % 32 != 0 || D != 16 || !d.global_scale || zp) return {};
         if ((reinterpret_cast<uintptr_t>(scale) & 1u) != 0) return {};
         p_dt = d.x_dtype;
-        k = fp4_observe_kernel(p_dt);
+        k = fp4_observe_kernel(p_dt, d.aux != nullptr);
+        zp = d.aux;   // the MSE mode's ct_mse_block (or none): this op has no zero point
     } else if (op == CT_OP_QUANTIZE_PACK_FP4) {
         if (d.x_dtype != CT_BF16 && d.x_dtype != CT_F16) return {};
         if (d.cols % 32 != 0 || !aligned16(scale) ) return {};
@@ -424,6 +426,29 @@ int run_batched(int op, int n, const ct_quant_desc* descs, const void* const* in
     return CT_OK;
 }
 
+// the checks of an MSE-mode call (d->aux = ct_mse_block) of the fused observer `op`, and the zeroed `any`: 1 when the streaming pass
+// should run, else the return code (CT_OK for an empty tensor; CT_E_UNSUPPORTED where only the generic path would take it)
+static int mse_prologue(int op, const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, void* out, int device, void* stream) {
+    if (device == CT_DEVICE_CPU || (reinterpret_cast<uintptr_t>(d->aux) & 7u) != 0) {
+        set_error("the MSE observer mode runs on a CUDA device with an 8-byte aligned ct_mse_block");
+        return CT_E_UNSUPPORTED;
+    }
+    int rc = validate_desc(d);
+    if (rc) return rc;
+    rc = check_dtypes(op, *d, zp_out != nullptr);
+    if (rc) return rc;
+    if (d->rows * d->cols == 0) return CT_OK;
+    if (!x || !scale_out || !out) { set_error("null tensor pointer"); return CT_E_ARG; }
+    const Plan p = op == CT_OP_OBSERVE_QUANTIZE_PACK ? plan_one(op, *d, x, scale_out, zp_out, nullptr, out) : plan_fp4(op, *d, x, scale_out, zp_out, nullptr, out);
+    if (!p.k.launch) return run_generic(op, *d, x, scale_out, zp_out, nullptr, out, nullptr);
+    rc = check_device(device);
+    if (rc) return rc;
+    DeviceGuard guard(device);
+    if (!guard.ok) return cuda_fail(cudaGetLastError(), "cudaSetDevice");
+    CT_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<uint8_t*>(d->aux) + offsetof(ct_mse_block, any), 0, sizeof(uint64_t), reinterpret_cast<cudaStream_t>(stream)));
+    return 1;
+}
+
 static int run_one(int op, const ct_quant_desc* d, const void* in, const void* scale, const void* zp,
                    const int32_t* g_idx, void* out, int device, void* stream) {
     if (!d) { set_error("null descriptor"); return CT_E_ARG; }
@@ -499,7 +524,13 @@ int ct_quantize_pack_fp4(const ct_quant_desc* d, const void* x, const void* scal
     return run_one(CT_OP_QUANTIZE_PACK_FP4, d, x, scale, zp, g_idx, packed, device, stream);
 }
 int ct_observe_quantize_pack_nvfp4(const ct_quant_desc* d, const void* x, void* scale_out_fp8, uint8_t* packed, int device, void* stream) {
-    return run_one(CT_OP_OBSERVE_QUANTIZE_PACK_FP4, d, x, scale_out_fp8, nullptr, nullptr, packed, device, stream);
+    if (!d || !d->aux) return run_one(CT_OP_OBSERVE_QUANTIZE_PACK_FP4, d, x, scale_out_fp8, nullptr, nullptr, packed, device, stream);
+    // MSE mode: the streaming pass with the search (local scales only; the global scale is an input), then the stop-step fix-up
+    int rc = mse_prologue(CT_OP_OBSERVE_QUANTIZE_PACK_FP4, d, x, scale_out_fp8, nullptr, packed, device, stream);
+    if (rc != 1) return rc;
+    rc = run_one(CT_OP_OBSERVE_QUANTIZE_PACK_FP4, d, x, scale_out_fp8, nullptr, nullptr, packed, device, stream);
+    if (rc) return rc;
+    return launch_mse_fixup_nvfp4(*d, x, scale_out_fp8, packed, reinterpret_cast<cudaStream_t>(stream));
 }
 int ct_unpack_dequantize_fp4(const ct_quant_desc* d, const uint8_t* packed, const void* scale, const void* zp, const int32_t* g_idx, void* out, int device, void* stream) {
     return run_one(CT_OP_UNPACK_DEQUANTIZE_FP4, d, packed, scale, zp, g_idx, out, device, stream);
@@ -548,10 +579,23 @@ int ct_sparse24_unpack_dequantize_int4(const ct_quant_desc* d, const int32_t* pa
     return run_one(CT_OP_SPARSE24_UNPACK_DEQUANTIZE, &t, packed, scale, zp, nullptr, out, device, stream);
 }
 int ct_observe_quantize_pack_int32(const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, int32_t* packed, int device, void* stream) {
-    return run_one(CT_OP_OBSERVE_QUANTIZE_PACK, d, x, scale_out, zp_out, nullptr, packed, device, stream);
+    if (!d || !d->aux) return run_one(CT_OP_OBSERVE_QUANTIZE_PACK, d, x, scale_out, zp_out, nullptr, packed, device, stream);
+    // MSE mode: the streaming pass with the search, then the stop-step fix-up; only the streaming kernel has the search
+    int rc = mse_prologue(CT_OP_OBSERVE_QUANTIZE_PACK, d, x, scale_out, zp_out, packed, device, stream);
+    if (rc != 1) return rc;
+    rc = run_one(CT_OP_OBSERVE_QUANTIZE_PACK, d, x, scale_out, zp_out, nullptr, packed, device, stream);
+    if (rc) return rc;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return launch_mse_fixup_pack(*d, x, scale_out, zp_out, packed, st);
 }
 int ct_batched(int op, int n, const ct_quant_desc* descs, const void* const* in, const void* const* scale,
                const void* const* zp, void* const* out, int device, void* stream) {
+    if (op == CT_OP_OBSERVE_QUANTIZE_PACK || op == CT_OP_OBSERVE_QUANTIZE_PACK_FP4 || op == CT_OP_OBSERVE_QUANTIZE_BLOCK || op == CT_OP_OBSERVE_QUANTIZE_MX)
+        for (int i = 0; i < n && descs; ++i)
+            if (descs[i].aux) {   // an MSE observer block: the whole-model observers run min-max only
+                set_error("ct_batched: tensor %d asks for the MSE observer (aux set); run it through its per-tensor entry point", i);
+                return CT_E_UNSUPPORTED;
+            }
     return run_batched(op, n, descs, in, scale, zp, nullptr, out, device, reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -261,6 +261,7 @@ extern "C" int ct_dynamic_fake_quantize(const ct_quant_desc* d, int asymmetric, 
         // ct_observe_tensor (kind 0) writes the scale and an asymmetric zero point; a symmetric scheme's zero point is a zero byte
         ct_quant_desc q = *d;
         q.global_scale = nullptr;
+        q.aux = nullptr;
         rc = ct_observe_tensor(&q, x, 0, scale_out, asym ? zp_out : nullptr, device, stream);
         if (rc) return rc;
         if (!asym) CT_CUDA_TRY(cudaMemsetAsync(zp_out, 0, 1, st));

@@ -15,9 +15,12 @@ StreamKernel bits_kernel(bool pack, int bits);                                  
 StreamKernel quant_kernel(int p_dt, bool fp8, int zp_kind, int max_unit);       // fast_quant.cu
 StreamKernel dequant_kernel(int p_dt, bool fp8, int zp_kind, bool f32_scale);   // f32_scale: fp8 codes, float32 scale, 16-bit output
 StreamKernel fake_kernel(int p_dt, int qtype, int bits, int zp_kind);           // fast_fake.cu
-StreamKernel observe_kernel(int p_dt, int bits, bool asym, int lanes_per_group); // fast_observe.cu
+StreamKernel observe_kernel(int p_dt, int bits, bool asym, int lanes_per_group, bool mse); // fast_observe.cu; mse: Job::aux = ct_mse_block
+// the MSE mode's stop-step fix-up after observe_kernel(..., mse = true) over the whole tensor of d (d.aux = ct_mse_block)
+int launch_mse_fixup_pack(const ct_quant_desc& d, const void* x, void* scale, void* zp, int32_t* packed, cudaStream_t st);
+int launch_mse_fixup_nvfp4(const ct_quant_desc& d, const void* x, void* scale, uint8_t* packed, cudaStream_t st);   // fast_fp4.cu
 StreamKernel fp4_quantpack_kernel(int p_dt, bool global_scale, int scale_dt, int zp_dt);   // fast_fp4.cu; zp_dt CT_NONE: no zero point
-StreamKernel fp4_observe_kernel(int p_dt);
+StreamKernel fp4_observe_kernel(int p_dt, bool mse);   // mse: Job::zp = ct_mse_block
 StreamKernel fp4_unpackdeq_kernel(int p_dt, int scale_dt);
 StreamKernel sparse24q_kernel(bool compress, int p_dt, int zp_kind);            // fast_sparse24q.cu: fused 2:4 select + int4
 

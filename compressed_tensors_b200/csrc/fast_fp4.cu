@@ -1,5 +1,7 @@
 // fast_fp4.cu -- streaming instantiations of the FP4 functors (fp4_ops.cuh) and the device-side exhaustive check of the
 // NVFP4 division shortcut.
+#include <algorithm>
+
 #include "engine.h"
 #include "fp4_ops.cuh"
 
@@ -30,10 +32,49 @@ StreamKernel fp4_quantpack_kernel(int p_dt, bool global_scale, int scale_dt, int
 }
 
 // NVFP4 observe + quantize + pack: the float8_e4m3fn scale is an OUTPUT
-StreamKernel fp4_observe_kernel(int p_dt) {
-    if (p_dt == CT_BF16) return stream_kernel<Fp4NvObserveQuantPackOp<BF16>>();
-    if (p_dt == CT_F16) return stream_kernel<Fp4NvObserveQuantPackOp<F16>>();
+StreamKernel fp4_observe_kernel(int p_dt, bool mse) {
+    if (p_dt == CT_BF16) return mse ? stream_kernel<Fp4NvObserveQuantPackOp<BF16, true>>() : stream_kernel<Fp4NvObserveQuantPackOp<BF16>>();
+    if (p_dt == CT_F16) return mse ? stream_kernel<Fp4NvObserveQuantPackOp<F16, true>>() : stream_kernel<Fp4NvObserveQuantPackOp<F16>>();
     return {};
+}
+
+// The NVFP4 MSE mode's second launch: the stop step from the call's `any` bits; a group of 16 whose mask has a bit above it is rewritten,
+// by one thread, with its last improving step <= S: its fp8 scale byte and its 8 bytes of nibbles, with the generic kernels' per-element
+// source (IEEE divisions, equal to the streaming shortcuts).  The global scale is an input and stays.
+template <class P>
+__global__ void __launch_bounds__(256) mse_fixup_nvfp4_kernel(const ct_mse_block* B, const void* x, const float* gsp, uint8_t* scale, uint8_t* packed,
+                                                              int64_t n_groups) {
+    const uint64_t keep = mse_keep(B);
+    const float gs = *gsp;
+    for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < n_groups; g += (int64_t)gridDim.x * blockDim.x) {
+        const uint64_t m = B->masks[g];
+        if ((m & ~keep) == 0) continue;
+        float amax = 0.f;   // a group that improved is finite
+        for (int j = 0; j < 16; ++j) amax = fmaxf(amax, fabsf(load_as_f32(x, g * 16 + j, P::DT)));
+        const float a = rnd_dt(amax * B->shrink[mse_last(m, keep)], P::DT);
+        uint32_t byte;
+        const float s = __fdiv_rn(obs_fp8_scale(__fmul_rn(gs, obs_round<P::DT>(__fdiv_rn(a, 6.0f))), byte), gs);
+        scale[g] = (uint8_t)byte;
+        for (int j = 0; j < 8; ++j) {
+            const float v0 = quant_scalar(load_as_f32(x, g * 16 + 2 * j, P::DT), s, false, 0.f, CT_F32, CT_Q_FP4, -6.f, 6.f);
+            const float v1 = quant_scalar(load_as_f32(x, g * 16 + 2 * j + 1, P::DT), s, false, 0.f, CT_F32, CT_Q_FP4, -6.f, 6.f);
+            packed[g * 8 + j] = (uint8_t)(fp4_nibble(v0) | (fp4_nibble(v1) << 4));
+        }
+    }
+}
+
+int launch_mse_fixup_nvfp4(const ct_quant_desc& d, const void* x, void* scale, uint8_t* packed, cudaStream_t st) {
+    const int64_t n_groups = d.rows * d.cols / 16;
+    if (n_groups == 0) return CT_OK;
+    const int64_t blocks = std::min<int64_t>((n_groups + 255) / 256, 4096);
+    const ct_mse_block* B = reinterpret_cast<const ct_mse_block*>(d.aux);
+    const float* gs = reinterpret_cast<const float*>(d.global_scale);
+    uint8_t* sc = reinterpret_cast<uint8_t*>(scale);
+    if (d.x_dtype == CT_BF16) mse_fixup_nvfp4_kernel<BF16><<<(unsigned)blocks, 256, 0, st>>>(B, x, gs, sc, packed, n_groups);
+    else mse_fixup_nvfp4_kernel<F16><<<(unsigned)blocks, 256, 0, st>>>(B, x, gs, sc, packed, n_groups);
+    count_launch();
+    CT_CUDA_TRY(cudaGetLastError());
+    return CT_OK;
 }
 
 // unpack + dequantize: the scale in the output dtype, or as stored (float8_e4m3fn / E8M0)

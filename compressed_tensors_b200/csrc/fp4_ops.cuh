@@ -11,6 +11,7 @@
 #pragma once
 
 #include "observe_core.cuh"
+#include "observe_mse.cuh"
 #include "ops.cuh"
 
 namespace ctb {
@@ -202,8 +203,10 @@ struct Fp4NvQuantPackOp {
 //   The global scale (generate_gparam over the whole tensor, helpers.py:308-337) is an INPUT: it needs a grid-wide reduction
 //   that has to finish before any group can be scaled.  Outputs: nibbles and the group scales as stored (float8_e4m3fn).
 // J.scale is written here (uint8 [n / 16]); J.aux = global scale.
+// MSE = true: J.zp (no zero point exists for this op) = the call's ct_mse_block; each group of 16 searches its max |x| shrink grid
+// (observe_mse.cuh) with the global scale fixed, and is written with its best improving step (mse_fixup_nvfp4_kernel applies the stop).
 // ------------------------------------------------------------------------------------
-template <class P>
+template <class P, bool MSE = false>
 struct Fp4NvObserveQuantPackOp {
     static constexpr int IN_BYTES = 16;
     static constexpr int GROUP = 4;
@@ -265,10 +268,42 @@ struct Fp4NvObserveQuantPackOp {
         float amax[2], s[2], rc[2];
         uint32_t codes = 0;
         bool slow = !tc.fast;
+        amax[0] = fmaxf(P::lo(g0), P::hi(g0));                                             // max(|min(min, 0)|, |max(max, 0)|) = max |x|
+        amax[1] = fmaxf(P::lo(g1), P::hi(g1));
+        if constexpr (MSE) {
+            ct_mse_block* B = reinterpret_cast<ct_mse_block*>(const_cast<void*>(J.zp));
+            const float norm = B->norm;
+            const bool square = norm == 2.0f;
+#pragma unroll
+            for (int g = 0; g < 2; ++g) {
+                // candidate i: max |x| of the shrunk range is T(max |x| * p_i); the scale as the reference forms it, IEEE divisions
+                auto partial = [&](float, float a) {
+                    uint32_t byte;
+                    const float cs = __fdiv_rn(group_scale<true>(a, tc.gs, byte), tc.gs);
+                    float e = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        if ((((k + off) >> 1) & 1) != g) continue;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const float xv = h ? P::hi(w[k][j]) : P::lo(w[k][j]);
+                                const float q = fp4_round(fminf(fmaxf(__fdiv_rn(xv, cs), -6.0f), 6.0f));
+                                e += mse_pow(rnd_dt(__fmul_rn(q, cs), P::DT) - xv, norm, square);
+                            }
+                    }
+                    return e;
+                };
+                const uint64_t gi = (uint64_t)(gc0 >> 1) + g;
+                uint64_t mask;
+                const int best = mse_search<P, 1>(B, 0.f, amax[g], partial, mask, B->errors ? B->errors + gi * B->steps : nullptr);
+                mse_publish(B, gi, mask);
+                amax[g] = rnd_dt(amax[g] * __ldg(&B->shrink[best]), P::DT);
+            }
+        }
 #pragma unroll
         for (int g = 0; g < 2; ++g) {
-            const uint32_t gm = g ? g1 : g0;
-            amax[g] = fmaxf(P::lo(gm), P::hi(gm));                                       // max(|min(min, 0)|, |max(max, 0)|) = max |x|
             // amax <= 2^14 also means clamp_x is the identity for every element of the group (chunk_fast<false> below)
             slow |= !(amax[g] <= 16384.0f && (amax[g] >= 9.094947017729282e-13f || amax[g] == 0.f));
             uint32_t byte;

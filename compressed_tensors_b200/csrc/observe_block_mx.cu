@@ -251,6 +251,8 @@ int run_observe_block_mx(int op, int n, const ct_quant_desc* descs, const void* 
                          int device, cudaStream_t st) {
     const bool block = op == CT_OP_OBSERVE_QUANTIZE_BLOCK;
     if (n < 0 || (n > 0 && (!descs || !in || !scale || !out))) { set_error("null table"); return CT_E_ARG; }
+    for (int i = 0; i < n; ++i)
+        if (descs[i].aux) { set_error("the fused BLOCK / MX observers have no MSE mode (aux set, tensor %d)", i); return CT_E_UNSUPPORTED; }
     if (device == CT_DEVICE_CPU) {
         set_error("the fused BLOCK / MX observers have no host twin; run the observer and the quantize separately");
         return CT_E_UNSUPPORTED;

@@ -9,12 +9,17 @@
 // Wider rows (up to CH_MAXC x 16384 columns) are split over the CTAs of one thread-block cluster: each CTA keeps its slice in
 // registers, the partial min / max meet in distributed shared memory, cluster rank 0 derives the qparams once and writes them into
 // every CTA's shared memory, and each CTA quantizes its own slice -- still one HBM read of the weight.
+// MSE mode (d->aux = ct_mse_block, per-row kernel only): between the row's min / max and its qparams the CTA runs the shrink-grid
+// search from the registers (observe_mse.cuh; the row's error is summed over the CTA with the warp shuffles and shared memory of the
+// min / max), writes the row with its best improving step, and mse_fixup_channel_kernel then applies the call's stop step.
 #include <cooperative_groups.h>
 #include <algorithm>
 #include <cstring>
 
 #include "engine.h"
+#include "generic.cuh"
 #include "observe_core.cuh"
+#include "observe_mse.cuh"
 #include "ops.cuh"
 
 namespace ctb {
@@ -24,9 +29,10 @@ constexpr int CH_MAXU = 8;   // most units (of 8 elements) per thread: rows up t
                              // 8 units so that short rows do not pay for registers they do not use (more CTAs resident per SM)
 constexpr int CH_MAXC = 8;   // most CTAs per cluster (the portable cluster size): rows up to 8 x 16384 = 131072 columns
 
-template <class P, int OUT, int ASYM, int MAXU>
+template <class P, int OUT, int ASYM, int MAXU, bool MSE = false>
 __global__ void __launch_bounds__(256) observe_channel_kernel(const uint4* __restrict__ x, void* __restrict__ scale_out, int8_t* __restrict__ zp_out,
-                                                              uint8_t* __restrict__ out, int64_t rows, int units /* cols / 8 */, const __grid_constant__ Common cm) {
+                                                              uint8_t* __restrict__ out, int64_t rows, int units /* cols / 8 */, const __grid_constant__ Common cm,
+                                                              ct_mse_block* B = nullptr) {
     __shared__ uint32_t red[2][8];
     __shared__ float qp[2];
     const int64_t r = blockIdx.x;
@@ -47,7 +53,56 @@ __global__ void __launch_bounds__(256) observe_channel_kernel(const uint4* __res
     }
     if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = mn2; red[1][threadIdx.x >> 5] = mx2; }
     __syncthreads();
-    if (threadIdx.x == 0) {
+    if constexpr (MSE) {
+        __shared__ float lh[2];
+        __shared__ float esum[2][8];
+        if (threadIdx.x == 0) {
+            for (int w = 1; w < 8; ++w) { mn2 = min2_nan<P>(mn2, red[0][w]); mx2 = max2_nan<P>(mx2, red[1][w]); }
+            obs_range2<P>(mn2, mx2, lh[0], lh[1]);
+        }
+        __syncthreads();
+        const float lo = lh[0], hi = lh[1], norm = B->norm;
+        const bool square = norm == 2.0f;
+        const int steps = B->steps;
+        float best = FLT_MAX;
+        int best_i = 0;
+        uint64_t mask = 0;
+        for (int i = 0; i < steps; ++i) {   // one barrier per step: the partial sums alternate between two rows of esum
+            const float p = __ldg(&B->shrink[i]);
+            float czq;
+            const float cs = obs_scale_zp<P::DT>(rnd_dt(lo * p, P::DT), rnd_dt(hi * p, P::DT), ASYM, cm.qmin, cm.qmax, czq);
+            const ScaleCtx c = make_scale_ctx(cs);
+            float e = 0.f;
+#pragma unroll
+            for (int u = 0; u < MAXU; ++u) {
+                if (u * 256 + (int)threadIdx.x >= units) continue;
+                const uint32_t w4[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    e += mse_elem<P, ASYM, OUT == CO_F8>(P::lo(w4[k]), cs, czq, c, cm.qmin, cm.qmax, norm, square) +
+                         mse_elem<P, ASYM, OUT == CO_F8>(P::hi(w4[k]), cs, czq, c, cm.qmin, cm.qmax, norm, square);
+            }
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) e += __shfl_xor_sync(0xffffffffu, e, d);
+            if ((threadIdx.x & 31) == 0) esum[i & 1][threadIdx.x >> 5] = e;
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                float t = esum[i & 1][0];
+                for (int w = 1; w < 8; ++w) t += esum[i & 1][w];
+                if (B->errors) B->errors[(size_t)r * steps + i] = t;
+                if (t < best) { best = t; best_i = i; mask |= 1ull << i; }   // NaN / inf never improve
+            }
+        }
+        if (threadIdx.x == 0) {
+            mse_publish(B, (uint64_t)r, mask);
+            const float p = __ldg(&B->shrink[best_i]);
+            float zq;
+            const float s = obs_scale_zp<P::DT>(rnd_dt(lo * p, P::DT), rnd_dt(hi * p, P::DT), ASYM, cm.qmin, cm.qmax, zq);
+            reinterpret_cast<unsigned short*>(scale_out)[r] = (unsigned short)P::from_float1(s);
+            if (ASYM) zp_out[r] = (int8_t)(int)zq;
+            qp[0] = s; qp[1] = zq;
+        }
+    } else if (threadIdx.x == 0) {
         for (int w = 1; w < 8; ++w) { mn2 = min2_nan<P>(mn2, red[0][w]); mx2 = max2_nan<P>(mx2, red[1][w]); }
         float lo, hi;
         obs_range2<P>(mn2, mx2, lo, hi);
@@ -201,8 +256,81 @@ static int chan_cluster_shape(int units, int& maxu) {
     return 0;
 }
 
+// The MSE mode's second launch, one CTA per row: the stop step from the call's `any` bits; a row whose mask has a bit above it is
+// rewritten with its last improving step <= S (min / max, calculate_qparams and codes with the generic kernels' per-element source,
+// equal to the streaming arithmetic); every other row only reads its mask.
+template <class P, int OUT, int ASYM>
+__global__ void __launch_bounds__(256) mse_fixup_channel_kernel(const ct_mse_block* B, const void* x, void* scale_out, int8_t* zp_out, uint8_t* out,
+                                                                int64_t cols, float qmin, float qmax) {
+    __shared__ float red[2][8];
+    __shared__ float qp[2];
+    const int64_t r = blockIdx.x;
+    const uint64_t keep = mse_keep(B), m = B->masks[r];
+    if ((m & ~keep) == 0) return;
+    const int best = mse_last(m, keep);
+    float mn = 0.f, mx = 0.f;   // min(min_vals, 0), max(max_vals, 0); a row that improved is finite
+    for (int64_t j = threadIdx.x; j < cols; j += 256) {
+        const float v = load_as_f32(x, r * cols + j, P::DT);
+        mn = fminf(mn, v);
+        mx = fmaxf(mx, v);
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, d));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, d));
+    }
+    if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = mn; red[1][threadIdx.x >> 5] = mx; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < 8; ++w) { mn = fminf(mn, red[0][w]); mx = fmaxf(mx, red[1][w]); }
+        const float p = B->shrink[best];
+        float zq;
+        const float s = obs_scale_zp<P::DT>(rnd_dt(mn * p, P::DT), rnd_dt(mx * p, P::DT), ASYM, qmin, qmax, zq);
+        reinterpret_cast<unsigned short*>(scale_out)[r] = (unsigned short)P::from_float1(s);
+        if (ASYM) zp_out[r] = (int8_t)(int)zq;
+        qp[0] = s; qp[1] = zq;
+    }
+    __syncthreads();
+    const float s = qp[0], zq = qp[1];
+    constexpr int QT = OUT == CO_F8 ? CT_Q_FLOAT : CT_Q_INT;
+    auto code = [&](int64_t j) { return quant_scalar(load_as_f32(x, r * cols + j, P::DT), s, ASYM, zq, P::DT, QT, qmin, qmax); };
+    if constexpr (OUT == CO_I8) {
+        for (int64_t j = threadIdx.x; j < cols; j += 256) reinterpret_cast<int8_t*>(out)[r * cols + j] = (int8_t)(int)code(j);
+    } else if constexpr (OUT == CO_F8) {
+        for (int64_t j = threadIdx.x; j < cols; j += 256) out[r * cols + j] = hd_f32_to_e4m3(code(j));
+    } else {
+        constexpr int BITS = OUT == CO_PACK4 ? 4 : 8;
+        uint32_t* words_out = reinterpret_cast<uint32_t*>(out) + r * cols * BITS / 32;
+        for (int64_t u = threadIdx.x * 32; u < cols; u += 256 * 32) {
+            const int nvalid = cols - u < 32 ? (int)(cols - u) : 32;
+            uint32_t words[BITS];
+            pack_group<BITS>(words, nvalid, [&](int j) { return (int32_t)code(u + j); });
+            for (int w = 0; w < (nvalid * BITS + 31) / 32; ++w) words_out[u * BITS / 32 + w] = words[w];
+        }
+    }
+}
+
+// the MSE mode: the per-row kernel with the search, then its fix-up (rows up to 256 * CH_MAXU units)
 template <class P, int OUT>
-static int launch_chan(bool asym, const uint4* x, void* s, int8_t* z, uint8_t* out, int64_t rows, int units, const Common& cm, cudaStream_t st) {
+static int launch_chan_mse(bool asym, const uint4* x, void* s, int8_t* z, uint8_t* out, int64_t rows, int units, const Common& cm, ct_mse_block* B,
+                           cudaStream_t st) {
+    const int per_thread = (units + 255) / 256;
+#define CT_CHAN_LAUNCH(A, U) observe_channel_kernel<P, OUT, A, U, true><<<(unsigned)rows, 256, 0, st>>>(x, s, z, out, rows, units, cm, B)
+    if (asym) { if (per_thread <= 2) CT_CHAN_LAUNCH(1, 2); else if (per_thread <= 4) CT_CHAN_LAUNCH(1, 4); else CT_CHAN_LAUNCH(1, 8); }
+    else { if (per_thread <= 2) CT_CHAN_LAUNCH(0, 2); else if (per_thread <= 4) CT_CHAN_LAUNCH(0, 4); else CT_CHAN_LAUNCH(0, 8); }
+#undef CT_CHAN_LAUNCH
+    CT_CUDA_TRY(cudaGetLastError());
+    if (asym) mse_fixup_channel_kernel<P, OUT, 1><<<(unsigned)rows, 256, 0, st>>>(B, x, s, z, out, (int64_t)units * 8, cm.qmin, cm.qmax);
+    else mse_fixup_channel_kernel<P, OUT, 0><<<(unsigned)rows, 256, 0, st>>>(B, x, s, z, out, (int64_t)units * 8, cm.qmin, cm.qmax);
+    count_launch(2);
+    CT_CUDA_TRY(cudaGetLastError());
+    return CT_OK;
+}
+
+template <class P, int OUT>
+static int launch_chan(bool asym, const uint4* x, void* s, int8_t* z, uint8_t* out, int64_t rows, int units, const Common& cm, cudaStream_t st,
+                       ct_mse_block* B) {
+    if (B) return launch_chan_mse<P, OUT>(asym, x, s, z, out, rows, units, cm, B, st);
     if (units > 256 * CH_MAXU) {
         int maxu = 0;
         const int csize = chan_cluster_shape(units, maxu);
@@ -223,12 +351,13 @@ static int launch_chan(bool asym, const uint4* x, void* s, int8_t* z, uint8_t* o
     return CT_OK;
 }
 template <class P>
-static int launch_chan_p(int outk, bool asym, const uint4* x, void* s, int8_t* z, uint8_t* out, int64_t rows, int units, const Common& cm, cudaStream_t st) {
+static int launch_chan_p(int outk, bool asym, const uint4* x, void* s, int8_t* z, uint8_t* out, int64_t rows, int units, const Common& cm, cudaStream_t st,
+                        ct_mse_block* B) {
     switch (outk) {
-    case CO_PACK4: return launch_chan<P, CO_PACK4>(asym, x, s, z, out, rows, units, cm, st);
-    case CO_PACK8: return launch_chan<P, CO_PACK8>(asym, x, s, z, out, rows, units, cm, st);
-    case CO_I8: return launch_chan<P, CO_I8>(asym, x, s, z, out, rows, units, cm, st);
-    default: return launch_chan<P, CO_F8>(false, x, s, z, out, rows, units, cm, st);
+    case CO_PACK4: return launch_chan<P, CO_PACK4>(asym, x, s, z, out, rows, units, cm, st, B);
+    case CO_PACK8: return launch_chan<P, CO_PACK8>(asym, x, s, z, out, rows, units, cm, st, B);
+    case CO_I8: return launch_chan<P, CO_I8>(asym, x, s, z, out, rows, units, cm, st, B);
+    default: return launch_chan<P, CO_F8>(false, x, s, z, out, rows, units, cm, st, B);
     }
 }
 
@@ -248,7 +377,13 @@ extern "C" int ct_observe_quantize_channel(const ct_quant_desc* d, const void* x
     else if (d->qtype == CT_Q_INT && d->q_dtype == CT_I8 && d->num_bits == 8) outk = CO_I8;
     else if (d->qtype == CT_Q_FLOAT && d->q_dtype == CT_F8E4M3 && d->num_bits == 8 && !asym) outk = CO_F8;
     const bool chan = d->rdiv == 1 && d->s_row_stride == 1 && (d->cdiv == CT_DIV_INF || d->cdiv >= d->cols);
-    const bool width_ok = d->cols <= 8LL * 256 * CH_MAXU * CH_MAXC;
+    // the MSE mode (d->aux) runs on the per-row kernel only: rows up to 16384 columns, on a device, with an 8-byte aligned block
+    ct_mse_block* B = reinterpret_cast<ct_mse_block*>(d->aux);
+    const bool width_ok = d->cols <= (B ? 8LL * 256 * CH_MAXU : 8LL * 256 * CH_MAXU * CH_MAXC);
+    if (B && (device == CT_DEVICE_CPU || (reinterpret_cast<uintptr_t>(B) & 7u) != 0 || !width_ok)) {
+        set_error("the channel observer's MSE mode runs on a CUDA device, rows up to %d columns, an 8-byte aligned ct_mse_block", 8 * 256 * CH_MAXU);
+        return CT_E_UNSUPPORTED;
+    }
     if (!dt_ok || outk < 0 || !chan || d->cols % 8 != 0 || !width_ok || d->rows > 0x7fffffffLL ||
         (asym && d->zp_dtype != CT_I8) || !aligned16(x) || !aligned16(out)) {
         set_error("fused channel observer supports bf16 / fp16 weights, cols %% 8 == 0, cols <= %d, int8 / fp8 codes or 4- / 8-bit packed int32, "
@@ -270,7 +405,8 @@ extern "C" int ct_observe_quantize_channel(const ct_quant_desc* d, const void* x
     };
     cm.qmin2 = bits16(cm.qmin); cm.qmax2 = bits16(cm.qmax); cm.bits = d->num_bits;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (B) CT_CUDA_TRY(cudaMemsetAsync(reinterpret_cast<uint8_t*>(B) + offsetof(ct_mse_block, any), 0, sizeof(uint64_t), st));
     const uint4* xp = reinterpret_cast<const uint4*>(x);
-    if (d->x_dtype == CT_BF16) return launch_chan_p<BF16>(outk, asym, xp, scale_out, reinterpret_cast<int8_t*>(zp_out), reinterpret_cast<uint8_t*>(out), d->rows, (int)(d->cols / 8), cm, st);
-    return launch_chan_p<F16>(outk, asym, xp, scale_out, reinterpret_cast<int8_t*>(zp_out), reinterpret_cast<uint8_t*>(out), d->rows, (int)(d->cols / 8), cm, st);
+    if (d->x_dtype == CT_BF16) return launch_chan_p<BF16>(outk, asym, xp, scale_out, reinterpret_cast<int8_t*>(zp_out), reinterpret_cast<uint8_t*>(out), d->rows, (int)(d->cols / 8), cm, st, B);
+    return launch_chan_p<F16>(outk, asym, xp, scale_out, reinterpret_cast<int8_t*>(zp_out), reinterpret_cast<uint8_t*>(out), d->rows, (int)(d->cols / 8), cm, st, B);
 }

@@ -159,6 +159,7 @@ extern "C" {
 int ct_observe_tensor(const ct_quant_desc* d, const void* x, int kind, void* scale_out, void* zp_out, int device, void* stream) {
     if (!d) { set_error("null descriptor"); return CT_E_ARG; }
     if (kind != 0 && kind != 1) { set_error("kind must be 0 (calculate_qparams) or 1 (generate_gparam)"); return CT_E_ARG; }
+    if (d->aux) { set_error("the per-tensor observer has no MSE mode (aux set)"); return CT_E_UNSUPPORTED; }
     int rc = check_device(device);
     if (rc) return rc;
     if (!x || !scale_out) { set_error("null tensor pointer"); return CT_E_ARG; }
@@ -169,6 +170,7 @@ int ct_observe_tensor(const ct_quant_desc* d, const void* x, int kind, void* sca
 
 int ct_observe_quantize_tensor(const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, void* q_out, int device, void* stream) {
     if (!d) { set_error("null descriptor"); return CT_E_ARG; }
+    if (d->aux) { set_error("the per-tensor observer has no MSE mode (aux set)"); return CT_E_UNSUPPORTED; }
     int rc = check_device(device);
     if (rc) return rc;
     if (!x || !scale_out || !q_out) { set_error("null tensor pointer"); return CT_E_ARG; }

@@ -3,7 +3,10 @@ CompressedTensorsQuantizer: a dense bf16 / fp16 checkpoint, or an FP8-block one 
 `weight_scale_inv` per 128 x 128 block, as DeepSeek-V3 / Kimi-K2 / Qwen3-FP8 ship them) -> a compressed-tensors checkpoint, shard by
 shard, without building the model.  Each targeted weight is calibrated with the memoryless min-max observer and compressed by ONE
 fused observer kernel on the job's device; the tensors written are exactly those the compressor of the inferred format writes
-(ModelCompressor.compress_model after calculate_qparams on the same min / max).
+(ModelCompressor.compress_model after calculate_qparams on the same min / max).  A scheme whose weights name observer "mse" /
+"memoryless_mse" is calibrated with the MSE shrink-grid search over each group's min / max instead (`ops.observe_*`; fused into the
+group, NVFP4 and per-row channel observer kernels, torch ops on the device otherwise), with the scheme's `observer_kwargs`; the
+NVFP4 global scale stays the min-max one, so fused siblings still share it.  The config records `observer` and `observer_kwargs`.
 
 NVFP4 siblings that a serving engine runs as one GEMM (q / k / v, gate / up, w1 / w3) share one weight_global_scale: the smallest
 of their per-tensor global scales, computed on the device.  `get_dependencies` makes the first member of each group (q_proj,
@@ -114,6 +117,7 @@ class CompressedTensorsQuantizer:
             raise ValueError(f"{name}: activation ordering needs calibration data")
         if self.scheme.weights.dynamic is not False:
             raise ValueError(f"{name}: weights must be quantized statically")
+        ops._mse_params(self.scheme.weights)   # an MSE observer's kwargs are checked before any shard is written
 
     def validate(self, tensors: dict[str, torch.Tensor]):
         self._check_scheme()

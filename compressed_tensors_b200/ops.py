@@ -1048,6 +1048,170 @@ def observe_tensor_gparam(x: torch.Tensor) -> torch.Tensor:
     return g
 
 
+# --------------------------------------------------------------------------------------------
+# MSE weight observer: a shrink-grid search over each group's min / max (observer "mse" / "memoryless_mse")
+# --------------------------------------------------------------------------------------------
+_MSE_OBSERVERS = ("mse", "memoryless_mse")
+_MSE_DEFAULTS = {"maxshrink": 0.20, "grid": 100.0, "patience": 5, "norm": 2.4}
+_FLT_MAX = float(torch.finfo(torch.float32).max)
+
+
+class _Mse(NamedTuple):
+    steps: int
+    patience: int
+    norm: float
+    shrink: tuple   # p_i = float32(1 - i / grid), i < steps
+
+
+def _mse_params(args) -> Optional[_Mse]:
+    """the search of an MSE observer from args.observer_kwargs, or None for every other observer"""
+    if getattr(args, "observer", None) not in _MSE_OBSERVERS:
+        return None
+    kw = dict(getattr(args, "observer_kwargs", None) or {})
+    unknown = sorted(set(kw) - set(_MSE_DEFAULTS))
+    if unknown:
+        raise ValueError(f"unknown MSE observer_kwargs {unknown}; expected a subset of {sorted(_MSE_DEFAULTS)}")
+    p = {**_MSE_DEFAULTS, **kw}
+    grid, maxshrink, norm = float(p["grid"]), float(p["maxshrink"]), float(p["norm"])
+    steps = int(maxshrink * grid) if math.isfinite(maxshrink * grid) else 0
+    if not 1 <= steps <= N.MSE_MAX_STEPS:
+        raise ValueError(f"MSE observer: int(maxshrink * grid) = {steps} steps, expected 1..{N.MSE_MAX_STEPS}")
+    patience = p["patience"]
+    if isinstance(patience, bool) or not isinstance(patience, (int, float)) or patience != int(patience) or patience < 1:
+        raise ValueError(f"MSE observer: patience must be an integer >= 1, got {patience!r}")
+    patience = int(patience)
+    if not math.isfinite(norm) or norm <= 0:
+        raise ValueError(f"MSE observer: norm must be finite and > 0, got {p['norm']}")
+    shrink = tuple(float(v) for v in torch.tensor([1 - i / grid for i in range(steps)], dtype=torch.float64).float())
+    return _Mse(steps, patience, norm, shrink)
+
+
+def _mse_choose(errors: torch.Tensor, mse: _Mse) -> Tuple[torch.Tensor, int]:
+    """the search rule on an error table [n_groups, steps]: (chosen step of every group, stop step S).  Step i improves a group when
+    its error is below min(FLT_MAX, every earlier error); S is the first step that ends `patience` steps in which no group of the
+    weight improved (steps - 1 if none); a group takes its last improving step <= S, or 0"""
+    e = errors.float().cpu()
+    best = torch.full((e.shape[0],), _FLT_MAX)
+    improved = torch.zeros(e.shape, dtype=torch.bool)
+    for i in range(mse.steps):
+        improved[:, i] = e[:, i] < best
+        best = torch.where(improved[:, i], e[:, i], best)
+    stop, run = mse.steps - 1, 0
+    for i, a in enumerate(improved.any(0).tolist()):
+        run = 0 if a else run + 1
+        if run >= mse.patience:
+            stop = i
+            break
+    idx = torch.arange(stop + 1)
+    chosen = torch.where(improved[:, :stop + 1], idx, -1).amax(1).clamp(min=0) if e.shape[0] else torch.zeros(0, dtype=torch.int64)
+    return chosen, stop
+
+
+def _mse_record(errors: torch.Tensor) -> None:
+    tables = getattr(_mode, "mse_tables", None)
+    if tables is not None:
+        tables.append(errors.float().cpu())
+
+
+class _mse_error_tables:
+    """test hook: every MSE search run inside the `with` appends its per-group error table [n_groups, steps] (float32, on the CPU) to
+    the yielded list, the kernel's own errors included"""
+
+    def __enter__(self) -> list:
+        self.prev = getattr(_mode, "mse_tables", None)
+        _mode.mse_tables = []
+        return _mode.mse_tables
+
+    def __exit__(self, *exc):
+        _mode.mse_tables = self.prev
+
+
+def _mse_aux(mse: _Mse, n_groups: int, device: torch.device):
+    """the device block of an MSE descriptor (ct_mse_block) and the buffers it points to; keep the tuple alive over the call"""
+    masks = torch.empty((n_groups,), dtype=torch.int64, device=device)
+    errors = torch.empty((n_groups, mse.steps), dtype=torch.float32, device=device) if getattr(_mode, "mse_tables", None) is not None else None
+    b = N.MseBlock(steps=mse.steps, patience=mse.patience, norm=mse.norm, any=0, masks=masks.data_ptr(),
+                   errors=errors.data_ptr() if errors is not None else None)
+    b.shrink[:mse.steps] = list(mse.shrink)
+    blk = torch.frombuffer(bytearray(bytes(b)), dtype=torch.uint8).to(device)
+    return blk, masks, errors
+
+
+def _observe_mse(xd: torch.Tensor, args, mse: _Mse, kind: str, qdt=None, global_scale=None):
+    """the MSE observer with torch ops on xd's device (any strategy, dtype or device): every candidate's qparams
+    (calculate_qparams of the shrunk min / max), its fake-quantized weight and the per-group sum of |fq - x|^norm in float32, then
+    the search rule and the min-max path's own output ops at each group's chosen candidate.
+      kind "codes" / "pack": (codes or packed words, scale, zero point or None)   "nvfp4": (packed, fp8 scale, global scale)
+      kind "mx": (codes or nibbles, E8M0 scale)"""
+    from .quantization.utils.helpers import calculate_qparams
+
+    strategy = _strategy_name(args)
+    rows, cols = xd.shape
+    if strategy in ("group", "tensor_group"):
+        g = int(getattr(args, "group_size"))
+        xr = xd.unflatten(-1, (-1, g))
+        mn, mx = xr.amin(-1), xr.amax(-1)
+
+        def gsum(e):
+            return e.unflatten(-1, (-1, g)).sum(-1)
+    elif strategy == "channel":
+        mn, mx = xd.amin(-1, keepdim=True), xd.amax(-1, keepdim=True)
+
+        def gsum(e):
+            return e.sum(-1, keepdim=True)
+    elif strategy == "tensor":
+        mn, mx = (t.reshape(1) for t in torch.aminmax(xd))
+
+        def gsum(e):
+            return e.sum().reshape(1)
+    elif strategy == "block":
+        bs = getattr(args, "block_structure", None)
+        if bs is None or len(bs) != 2:
+            raise ValueError("block quantization needs a block_structure [rows, cols]")
+        bh, bw = int(bs[0]), int(bs[1])
+        nrb, ncb = -(-rows // bh), -(-cols // bw)
+
+        def blocks(t):   # zero padding is neutral for min / max (the rule clamps min <= 0 <= max) and for the error sums
+            return torch.nn.functional.pad(t, (0, ncb * bw - cols, 0, nrb * bh - rows)).reshape(nrb, bh, ncb, bw)
+        mn, mx = blocks(xd).amin(dim=(1, 3)), blocks(xd).amax(dim=(1, 3))
+
+        def gsum(e):
+            return blocks(e).sum(dim=(1, 3))
+    else:
+        raise NotImplementedError(f"the MSE observer does not support strategy {strategy}")
+    symmetric = bool(getattr(args, "symmetric", True))
+    xf = xd.float()
+    if kind == "nvfp4" and getattr(args, "scale_dtype", None) is None:
+        # NVFP4 stores its group scales as float8_e4m3fn: every candidate is judged with the scale it would be stored with
+        args = args.model_copy(update={"scale_dtype": torch.float8_e4m3fn})
+
+    def qparams(p):   # calculate_qparams of min / max shrunk by p (torch's tensor * python float: float32 product, rounded to x's dtype)
+        scale, zp = calculate_qparams((mn.float() * p).to(mn.dtype), (mx.float() * p).to(mx.dtype), args, global_scale=global_scale)
+        return scale, (None if symmetric else zp)
+
+    table = []
+    for p in mse.shrink:
+        scale, zp = qparams(p)
+        d = (fake_quantize(xd, scale, zp, args, global_scale=global_scale).float() - xf).abs()
+        table.append(gsum(d * d if mse.norm == 2.0 else d.pow(mse.norm)).reshape(-1))
+    errors = torch.stack(table, 1)
+    _mse_record(errors)
+    chosen, _ = _mse_choose(errors, mse)
+    p = torch.tensor(mse.shrink, dtype=torch.float32)[chosen].reshape(mn.shape).to(xd.device)
+    scale, zp = qparams(p)
+    if kind == "nvfp4":
+        return quantize_pack_fp4(xd, scale, None, args, global_scale=global_scale), scale.to(torch.float8_e4m3fn), global_scale
+    if kind == "mx":
+        out = quantize_pack_fp4(xd, scale, None, args) if int(args.num_bits) == 4 else quantize(xd, scale, None, args, dtype=torch.float8_e4m3fn)
+        return out, compress_mx_scale(scale, torch.uint8)
+    out = quantize_pack(xd, scale, zp, args) if kind == "pack" else quantize(xd, scale, zp, args, dtype=qdt)
+    return out, scale, zp
+
+
+def _back_all(outs, x):
+    return tuple(_back(t, x) if t is not None else None for t in outs)
+
+
 @torch.no_grad()
 def observe_quantize_pack(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
     """Memoryless min-max observer + quantize + pack in ONE pass over the weight (SURVEY 8(f) rank 1):
@@ -1069,16 +1233,26 @@ def observe_quantize_pack(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Te
     fused_ok = (qtype == N.Q_INT and strategy == "group" and group in (32, 64, 128, 256) and cols % group == 0
                 and x.dtype in (torch.bfloat16, torch.float16) and bits in (4, 8) and (cols * bits) % 32 == 0
                 and (rows * cols) % 32 == 0)
-    if fused_ok:
+    mse = _mse_params(args) if x.numel() > 0 else None
+    if fused_ok and (mse is None or idx != _CPU):
         ng = cols // group
         scale = torch.empty((rows, ng), dtype=x.dtype, device=xd.device)
         zp = None if symmetric else torch.empty((rows, ng), dtype=torch.int8, device=xd.device)
         packed = torch.empty((rows, cols * bits // 32), dtype=torch.int32, device=xd.device)
         d = _qdesc(rows, cols, 1, group, ng, qtype, bits, x_dtype=x.dtype, scale_dtype=x.dtype, compute_dtype=x.dtype,
                    zp_dtype=None if symmetric else torch.int8, q_dtype=torch.int8)
+        aux = None
+        if mse is not None:
+            aux = _mse_aux(mse, rows * ng, xd.device)
+            d.aux = aux[0].data_ptr()
         rc = N.lib().ct_observe_quantize_pack_int32(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(packed), idx, N.stream_ptr(idx))
-        N.check(rc, "observe_quantize_pack")
-        return _back(packed, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+        if not (mse is not None and rc == N.CT_E_UNSUPPORTED):   # an MSE search the kernel declines runs with torch ops below
+            N.check(rc, "observe_quantize_pack")
+            if aux is not None and aux[2] is not None:
+                _mse_record(aux[2])
+            return _back(packed, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+    if mse is not None:
+        return _back_all(_observe_mse(xd, args, mse, "pack"), x)
     return _observe_unfused("observe_quantize_pack", x, xd, args, group, True, torch.int32)
 
 
@@ -1131,13 +1305,22 @@ def observe_quantize_pack_nvfp4(x: torch.Tensor, args, global_scale: Optional[to
     else:
         gs = generate_gparam(xd.min(), xd.max())
     gs = gs.reshape(1).to(torch.float32).contiguous()
-    if x.dtype in (torch.bfloat16, torch.float16) and cols % 32 == 0 and rows > 0:
+    mse = _mse_params(args) if x.numel() > 0 else None
+    if x.dtype in (torch.bfloat16, torch.float16) and cols % 32 == 0 and rows > 0 and (mse is None or idx != _CPU):
         scale = torch.empty((rows, cols // 16), dtype=torch.float8_e4m3fn, device=xd.device)
         packed = torch.empty((rows, cols // 2), dtype=torch.uint8, device=xd.device)
         d = _nvfp4_observe_desc(rows, cols, x.dtype, gs.data_ptr())
+        aux = _mse_aux(mse, rows * cols // 16, xd.device) if mse is not None else None
+        if aux is not None:
+            d.aux = aux[0].data_ptr()
         rc = N.lib().ct_observe_quantize_pack_nvfp4(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(packed), idx, N.stream_ptr(idx))
-        N.check(rc, "observe_quantize_pack_nvfp4")
-        return _back(packed, x), _back(scale, x), _back(gs, x)
+        if not (mse is not None and rc == N.CT_E_UNSUPPORTED):   # an MSE search the kernel declines runs with torch ops below
+            N.check(rc, "observe_quantize_pack_nvfp4")
+            if aux is not None and aux[2] is not None:
+                _mse_record(aux[2])
+            return _back(packed, x), _back(scale, x), _back(gs, x)
+    if mse is not None:
+        return _back_all(_observe_mse(xd, args, mse, "nvfp4", global_scale=gs), x)
     g = xd.unflatten(-1, (-1, 16))
     scale, _ = calculate_qparams(g.amin(-1), g.amax(-1), args, global_scale=gs)
     packed = quantize_pack_fp4(xd, scale, None, args, global_scale=gs)
@@ -1184,6 +1367,9 @@ def _observe_quantize_block(x: torch.Tensor, args, qtype: int, bits: int, symmet
         return (torch.empty((rows, cols), dtype=qdt, device="meta"), torch.empty((nrb, ncb), dtype=x.dtype, device="meta"), zp)
     idx = _dev_index(x)
     xd = _to_dev(x, idx).contiguous()
+    mse = _mse_params(args) if x.numel() > 0 else None
+    if mse is not None:
+        return _back_all(_observe_mse(xd, args, mse, "codes", qdt), x)
     if (idx != _CPU and qtype == N.Q_FLOAT and bits == 8 and symmetric and x.dtype in (torch.bfloat16, torch.float16)
             and cols % 8 == 0 and bw % 8 == 0 and rows * cols > 0 and _aligned(xd)):
         scale = torch.empty((nrb, ncb), dtype=x.dtype, device=xd.device)
@@ -1235,6 +1421,9 @@ def observe_quantize_mx(x: torch.Tensor, args) -> Tuple[torch.Tensor, torch.Tens
         return torch.empty(q_shape, dtype=q_dt, device="meta"), torch.empty((rows, cols // 32), dtype=torch.uint8, device="meta")
     idx = _dev_index(x)
     xd = _to_dev(x, idx).contiguous()
+    mse = _mse_params(args) if x.numel() > 0 else None
+    if mse is not None:
+        return _back_all(_observe_mse(xd, args, mse, "mx"), x)
     if idx != _CPU and x.dtype in (torch.bfloat16, torch.float16) and rows * cols > 0 and _aligned(xd):
         scale = torch.empty((rows, cols // 32), dtype=torch.uint8, device=xd.device)
         out = torch.empty(q_shape, dtype=q_dt, device=xd.device)
@@ -1262,7 +1451,9 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
       GROUP + pack               : `observe_quantize_pack`
       BLOCK (FP8_BLOCK)          : `ct_observe_quantize_block` -- one CTA per block: min / max, calculate_qparams, fp8 codes; returns
                                    (float8_e4m3fn [R, C], scale in x.dtype [ceil(R / bh), ceil(C / bw)], None)
-    Everything else runs the observer with torch reductions on the device and then the quantize kernel."""
+    Everything else runs the observer with torch reductions on the device and then the quantize kernel.
+    args.observer "mse" / "memoryless_mse" runs the MSE shrink-grid search instead: fused into the GROUP + pack kernel and the per-row
+    CHANNEL kernel (rows up to 16384 columns), torch ops on the device (`_observe_mse`) for everything else."""
     qtype, bits = _qparams(args)
     strategy = _strategy_name(args)
     symmetric = bool(getattr(args, "symmetric", True))
@@ -1278,18 +1469,26 @@ def observe_quantize(x: torch.Tensor, args, pack: bool = False) -> Tuple[torch.T
     idx = _dev_index(x)
     xd = _to_dev(x, idx).contiguous()
     qdt = torch.int32 if pack else (torch.float8_e4m3fn if qtype == N.Q_FLOAT else torch.int8)
+    mse = _mse_params(args) if x.numel() > 0 else None
     fused_ok = (strategy == "channel" and x.dtype in (torch.bfloat16, torch.float16) and cols % 8 == 0 and cols > 0 and rows > 0
                 and qtype in (N.Q_INT, N.Q_FLOAT) and (bits in (4, 8) if pack else bits == 8) and (symmetric or qtype == N.Q_INT))
-    if fused_ok:
+    if fused_ok and (mse is None or idx != _CPU):
         scale = torch.empty((rows, 1), dtype=x.dtype, device=xd.device)
         zp = None if symmetric else torch.empty((rows, 1), dtype=torch.int8, device=xd.device)
         out = torch.empty((rows, cols * bits // 32) if pack else (rows, cols), dtype=qdt, device=xd.device)
         d = _qdesc(rows, cols, 1, N.INF, 1, qtype, bits, x_dtype=x.dtype, scale_dtype=x.dtype, compute_dtype=x.dtype,
                    zp_dtype=None if symmetric else torch.int8, q_dtype=qdt)
+        aux = _mse_aux(mse, rows, xd.device) if mse is not None else None
+        if aux is not None:
+            d.aux = aux[0].data_ptr()
         rc = N.lib().ct_observe_quantize_channel(ctypes.byref(d), N.ptr(xd), N.ptr(scale), N.ptr(zp), N.ptr(out), idx, N.stream_ptr(idx))
-        if rc != N.CT_E_UNSUPPORTED:   # declined (a row wider than one cluster holds): the unfused path below
+        if rc != N.CT_E_UNSUPPORTED:   # declined (a row wider than the kernel holds): the unfused path below
             N.check(rc, "observe_quantize")
+            if aux is not None and aux[2] is not None:
+                _mse_record(aux[2])
             return _back(out, x), _back(scale, x), (_back(zp, x) if zp is not None else None)
+    if mse is not None:
+        return _back_all(_observe_mse(xd, args, mse, "pack" if pack else "codes", qdt), x)
     if (strategy == "tensor" and _tensor_observer_ok(xd) and qtype in (N.Q_INT, N.Q_FLOAT) and (symmetric or qtype == N.Q_INT)
             and (bits in (4, 8) if pack else bits == 8) and (not pack or (cols * bits) % 32 == 0)):
         # ONE call: grid-wide min / max -> calculate_qparams on the device -> quantize (or quantize + pack) with the device-resident scale

@@ -206,6 +206,36 @@ int ct_unpack_dequantize_int32(const ct_quant_desc* d, const int32_t* packed, co
 int ct_observe_quantize_pack_int32(const ct_quant_desc* d, const void* x, void* scale_out, void* zp_out, int32_t* packed,
                                    int device, void* stream);
 
+/* MSE observer mode of ct_observe_quantize_pack_int32 (and of the NVFP4 and channel observers, below): d->aux != NULL points to this block, in DEVICE memory.  Every group's
+ * min / max is shrunk by each p_i, i < steps (lo = T(min * p_i), hi = T(max * p_i) in x's dtype T), calculate_qparams gives the
+ * candidate's scale / zero point, and the group's error e(i) = sum |fake_quantize(x) - x|^norm is formed in float32 (d * d for
+ * norm == 2, exp2(norm * log2|d|) otherwise).  Step i improves a group when e(i) < min(FLT_MAX, e(0 .. i-1)); the search stops at
+ * the first step S ending `patience` steps in which no group of the call improved (steps - 1 if none), and every group is written
+ * with the qparams of its last improving step <= S (step 0, the min-max qparams, if none).
+ *   shrink[i]  p_i = float32(1 - i / grid), computed on the host
+ *   any        bit i set when some group improved at step i; the entry point zeroes it
+ *   masks      uint64 [rows * cols / group] scratch: each group's improvement bits (written)
+ *   errors     float32 [rows * cols / group, steps] or NULL: every e(i) (written when given)
+ * The kernel writes each group's best improving step over all steps; a second launch computes S on the device and rewrites only
+ * the groups whose mask has a bit above S.  No host synchronisation.  Same shapes and limits as the min-max mode; anything else
+ * (and device = CT_DEVICE_CPU) returns CT_E_UNSUPPORTED.  The block is read on the device and not checked: it must hold a valid
+ * `steps` and `masks`.
+ * ct_observe_quantize_pack_nvfp4 and ct_observe_quantize_channel take the same block: NVFP4 searches each group of 16's max |x| with
+ * the global scale fixed (masks / errors per group of 16); CHANNEL searches each row (masks / errors per row) on rows up to 16384
+ * columns.  ct_observe_quantize_block, ct_observe_quantize_mx, ct_observe_tensor / _quantize_tensor and ct_batched's observer ops
+ * return CT_E_UNSUPPORTED when d->aux is set. */
+#define CT_MSE_MAX_STEPS 64
+typedef struct ct_mse_block {
+    float shrink[CT_MSE_MAX_STEPS];
+    int32_t steps;          /* 1 .. CT_MSE_MAX_STEPS */
+    int32_t patience;       /* >= 1 */
+    float norm;             /* finite, > 0 */
+    int32_t _reserved;
+    uint64_t any;
+    uint64_t* masks;
+    float* errors;
+} ct_mse_block;
+
 /* ---- FP4 (E2M1) and MX formats (SURVEY.md 8(f) rank 2) -------------------------
  * cast_to_fp4: quantization/utils/fp4_utils.py:77-98 (x and out share a float dtype).
  * pack_fp4 / unpack_fp4: compressors/nvfp4/helpers.py:108-158 / :162-193 -- x [rows, cols] of VALID fp4 values
